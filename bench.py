@@ -2,7 +2,8 @@
 """bench.py — env steps/s of the batched connect_four ApplyAction hot path (BASELINE.json configs[1]).
 
   python bench.py --gpus N --steps K --warmup W          # our arm (CUDA, through the C ABI)
-  python bench.py --impl reference --gpus N ...          # the CPU arm on the box's host cores
+  python bench.py --impl reference --gpus N ...          # the CPU arm on the host cores
+  python bench.py ... --dump-outputs DIR                 # also write what the last timed step computed, as .npy
 
 One "step" = one pass of State::ApplyAction over one batch of 1,048,576 connect_four states (SoA, 16 B per
 state) with one legal action per state.  The (state, action) stream is synthetic: every lane is advanced
@@ -44,7 +45,7 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback: H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
 
 
 # ------------------------------------------------------------------------------------------------ CPU arm
@@ -214,6 +215,26 @@ def build_workload(torch, game, n, dev, seed, with_history=False):
     return game, snap, actions.contiguous()
 
 
+DUMP_SAMPLE = 4096          # lanes whose observation tensor is dumped (a fixed, seeded sample)
+
+
+def dump_outputs(out_dir, torch, batch):
+    """What a caller of the timed path reads back from the batch it stepped, as DIR/<name>.npy: the state of every lane
+    (player to move, terminal flag, returns, legal-action mask word) and the observation tensor of a fixed, seeded sample
+    of lanes.  ~26 MB in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    cur, term, rets = batch.status()
+    mask = batch.legal_actions_mask_words()
+    lanes = np.sort(np.random.default_rng(0).choice(batch.n, DUMP_SAMPLE, replace=False))
+    obs = batch.observation_tensor(player=0)[torch.from_numpy(lanes).to(mask.device)]
+    arrays = {"current_player": cur.float(), "terminal": term.float(), "returns": rets.float(),
+              "legal_mask_word": mask.to(torch.int64).bitwise_and(0xFFFFFFFF).double(),
+              "observation_sample": obs.float(), "observation_sample_lanes": torch.from_numpy(lanes).double()}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy())
+
+
 def run_gpu(args):
     import torch
     import open_spiel_b200 as b2
@@ -239,7 +260,7 @@ def run_gpu(args):
     game = b2.Game("connect_four", device=local)
     _, snap, actions0 = build_workload(torch, game, n, dev, seed=0x5EED + rank)
     # "Inputs larger than L2": every timed step owns a private copy of the 16 MiB batch and of the 4 MiB action
-    # array ((K+W) x 20 MiB in total, far beyond the 126 MB L2), so no step can find its lines cached; in steady
+    # array ((K+W) x 20 MiB in total, far beyond the H100's 50 MB L2), so no step can find its lines cached; in steady
     # state each step reads 20 MiB from HBM and leaves 16 MiB of dirty lines for later eviction — exactly the
     # algorithmic traffic.  Nothing but the K apply launches sits between the two timing events.
     C = min(K, 512)                   # timed launches per graph; larger K runs ceil(K/C) graphs, restoring between
@@ -340,6 +361,8 @@ def run_gpu(args):
     ms_apply_total = time_graphs(lambda i: works[i].apply_actions(acts[i]), n_streams=2)
     for w_ in works:
         w_.check_errors()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, torch, works[W + (K - 1) % C])     # the batch the last timed launch stepped
     ms_apply_s1 = time_graphs(lambda i: works[i].apply_actions(acts[i]), reps=2, n_streams=1)
     ms_apply_s4 = time_graphs(lambda i: works[i].apply_actions(acts[i]), reps=2, n_streams=4)
     for w_ in works:
@@ -446,9 +469,9 @@ def run_gpu(args):
         torch.cuda.empty_cache()
         return res
 
-    loops["mcts_go9x9"] = mcts_line(65536, 128)          # throughput grows with resident trees until ~14 warps/SM (DESIGN.md §4)
-    # deep trees (BASELINE configs[2] is 100k sims/move; a full 100k-sim run of enough trees takes minutes and is recorded
-    # in profiles/): steady state at 10k simulations per tree, where descents are ~10 levels deep
+    loops["mcts_go9x9"] = mcts_line(65536, 128)          # throughput grows with resident trees (DESIGN.md §4)
+    # deep trees (BASELINE configs[2] is 100k sims/move; a full 100k-sim run of enough trees takes minutes): steady state
+    # at 10k simulations per tree, where descents are ~10 levels deep
     loops["mcts_go9x9_deep"] = mcts_line(args.deep_trees, args.deep_sims, nodes=args.deep_trees * 240000)
     # self-play rollouts: breakthrough 8x8, 2^20 games per GPU, statistics all-reduced
     bt = b2.Game("breakthrough", device=local)
@@ -529,16 +552,6 @@ def run_gpu(args):
     cores = os.cpu_count() or 1
     cpu_v, cpu_kind, cpu_per = cpu_arm(1 << 18, 1, 8)
     cpu_secs = sum(cpu_per)
-    traffic, traffic_src = None, None
-    for name in ("r02_apply_traffic.json", "r01_apply_traffic.json"):       # ncu --set full capture of this kernel (not measured in-run)
-        tp = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tp):
-            try:
-                traffic = json.load(open(tp)).get("dram_bytes_per_launch")
-                traffic_src = "profiles/" + name + " (ncu dram__bytes_read.sum + dram__bytes_write.sum of one launch; constant, not re-measured by this run)"
-                break
-            except Exception:
-                pass
 
     def frac(ms):
         return BYTES_APPLY * n / (ms / 1e3) / 1e9 / peak
@@ -564,16 +577,15 @@ def run_gpu(args):
                                      "cfr_leduc_iters": loops["cfr_leduc"]["iters"],
                                      "rollouts_breakthrough_games_per_s": loops["rollouts_breakthrough"]["games_per_s"]}},
         "roofline": {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                     "traffic": traffic, "traffic_source": traffic_src, "kernel": "k_apply<ConnectFourRules,4>",
+                     "kernel": "k_apply<ConnectFourRules,4>",
                      "bytes_per_step": BYTES_APPLY, "peak_source": peak_src,
                      "frac_1_chain": frac(ms_apply_s1 / K), "frac_4_chains": frac(ms_apply_s4 / K),
                      "frac_64M_lanes": BYTES_APPLY * big_n / (ms_big / 1e3) / 1e9 / peak,
                      "note": "achieved = 36 B x 1,048,576 lanes / (elapsed / K).  1M lanes are 5.7 us of pure transfer per launch: launches "
                              "ordered one after the other on a single chain pay a grid ramp + drain each (frac_1_chain, round 1's figure); "
                              "declared independent — they are: different batches — consecutive launches overlap (frac, frac_4_chains); one "
-                             "launch over 64M lanes (> L2) is frac_64M_lanes.  The timed region as a whole pays one ramp-up and one drain "
-                             "(~8 us, the same with the timing events as graph nodes: profiles/r02_bench_k20.json), i.e. frac ~0.93 at "
-                             "--steps 20 and ~0.998 at --steps 200"},
+                             "launch over 64M lanes (> L2) is frac_64M_lanes.  The timed region as a whole pays one ramp-up and one "
+                             "drain, so frac grows with --steps"},
         "cpu_baseline": {"value": cpu_v, "unit": UNIT, "cores": 1, "kind": cpu_kind,
                          "sample": "%d states x 8 passes, 1 thread, Clone excluded (%.2f s timed)" % (1 << 18, cpu_secs),
                          "host_cores": cores},
@@ -613,9 +625,12 @@ def main():
     ap.add_argument("--deep-trees", type=int, default=8192, help="trees per GPU of the deep MCTS line")
     ap.add_argument("--deep-sims", type=int, default=10000, help="simulations per tree of the deep MCTS line")
     ap.add_argument("--cfr-iters", type=int, default=100000, help="CFRSolver iterations (BASELINE configs[3]: 100k)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed ApplyAction step computed to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes the device arm's outputs; it does not apply to --impl reference")
         return run_reference(args)
     return run_gpu(args)
 

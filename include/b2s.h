@@ -1,10 +1,10 @@
-/* b2s.h — C ABI of the B200-native batched game-simulation and search engine.
+/* b2s.h — C ABI of the H100-native batched game-simulation and search engine.
  *
  * This is the drop-in boundary for ONE hot path of google-deepmind/open_spiel: the per-game
  * State transition functions (ApplyAction / LegalActions / IsTerminal / Returns /
  * ObservationTensor) of tic_tac_toe, connect_four, breakthrough, hex, go, kuhn_poker and
  * leduc_poker, and the MCTSBot / CFRSolver loops that drive them.  Everything here runs as
- * hand-written sm_100a CUDA over struct-of-arrays batches of packed states resident in HBM.
+ * hand-written sm_90a CUDA over struct-of-arrays batches of packed states resident in HBM.
  * There is no CPU fallback: every entry point fails (non-zero status) when no CUDA device exists.
  *
  * Shape follows the reference's own C-ABI precedent, open_spiel/go/go_open_spiel.h:21-70

@@ -1,4 +1,4 @@
-"""open_spiel_b200 — B200-native batched game simulation + search behind OpenSpiel's State/Game API.
+"""open_spiel_b200 — H100-native batched game simulation + search behind OpenSpiel's State/Game API.
 
 Host-side mirror of the reference's Python surface for the hot path (python/pybind11/pyspiel.cc:355-476,
 720-735): load_game, Game.new_initial_state, State.{apply_action, legal_actions, ...}, plus the batched

@@ -8,7 +8,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# B2S_LIBRARY: another build of the same C ABI (A/B kernel measurements, scripts/r02_item9.sh); still a CUDA library, not a fallback
+# B2S_LIBRARY: another build of the same C ABI (A/B kernel measurements); still a CUDA library, not a fallback
 SO_PATH = os.environ.get("B2S_LIBRARY") or os.path.join(_HERE, "libb2s.so")
 
 

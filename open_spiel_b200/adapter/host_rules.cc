@@ -1,5 +1,5 @@
 // Host instantiation of the b2s rule cores for the scalar State adapter (see host_rules.h).
-// Everything game-specific below is a call into open_spiel_b200/csrc/rules_<game>.cuh — the source the sm_100a kernels
+// Everything game-specific below is a call into open_spiel_b200/csrc/rules_<game>.cuh — the source the sm_90a kernels
 // are instantiated from — through the one-lane Ctx the kernels use (cap = 1: the SoA planes of a single lane are
 // contiguous, which is exactly the b2s_state_get blob layout).
 #include "host_rules.h"

@@ -1,7 +1,7 @@
 // Scalar (one State) execution of the b2s rule cores on the host, for the open_spiel::State adapter.
 //
 // SURVEY §8(b)(i): "scalar State methods run the same __host__ __device__ rule core on the CPU and keep history_ via
-// the base class".  host_rules.cc compiles open_spiel_b200/csrc/rules_*.cuh — the exact source the sm_100a kernels are
+// the base class".  host_rules.cc compiles open_spiel_b200/csrc/rules_*.cuh — the exact source the sm_90a kernels are
 // instantiated from — with the host compiler, so a single open_spiel::State never pays a kernel launch + PCIe round
 // trip per method call.  This is NOT a CPU fallback of the batched path: there is no batched entry point here, and
 // every batched call (b2s_apply_actions, b2s_step_fused, b2s_mcts_search, b2s_cfr_iterate, ...) exists only in

@@ -33,7 +33,7 @@ struct HostPipe {                 // per device: b2s_step_fused_host's upload+ke
   cudaEvent_t ev[8] = {};
 };
 static HostPipe g_host_pipe[kMaxDevices];
-constexpr int kHostChunks = 8, kHostChunksDefault = 2;   // measured on B200 + PCIe gen5: 1: 0.364 ms, 2: 0.343, 4: 0.358, 8: 0.395 (1M lanes)
+constexpr int kHostChunks = 8, kHostChunksDefault = 2;   // B2S_HOST_CHUNKS overrides (scripts/e2e_chunks.py measures each)
 
 struct Batch {
   GameOps* ops = nullptr;
@@ -114,7 +114,7 @@ using namespace b2s;
 extern "C" {
 
 const char* b2s_last_error(void) { return g_err.c_str(); }
-const char* b2s_version(void) { return "b2s 0.1 (sm_100a)"; }
+const char* b2s_version(void) { return "b2s 0.1 (sm_90a)"; }
 int64_t b2s_launch_count(void) { return g_launches; }
 static int64_t g_host_graph_launches = 0, g_host_zero_copy_steps = 0;
 int64_t b2s_host_graph_launches(void) { return g_host_graph_launches; }
@@ -378,8 +378,7 @@ static int step_host_impl(Batch* B, const void* actions_h, int action_bytes, uin
   static const bool graphs_on = [] { const char* e = getenv("B2S_HOST_GRAPH"); return !e || atoi(e) != 0; }();
 
   // two chunks overlap the upload + kernel of one half with the download of the other; that only pays when the copies
-  // are long compared with the fixed cost of a copy (~10-15 us of DMA set-up each, measured with the copies as graph nodes
-  // too: scripts/r02_e2e_graph.py): below ~4 MiB of traffic the call runs as one chunk
+  // are long compared with the fixed DMA set-up cost of a copy: below ~4 MiB of traffic the call runs as one chunk
   const int n_chunks = env_chunks ? env_chunks : kHostChunksDefault;
   const bool split = n_chunks > 1 && n >= (1 << 18) && (env_chunks || bytes_per_lane * (size_t)n >= (4u << 20));
   const int chunks = split ? n_chunks : 1;
@@ -406,10 +405,9 @@ static int step_host_impl(Batch* B, const void* actions_h, int action_bytes, uin
 
   // ---- graph path: the pipeline is ONE cudaGraphLaunch -----------------------------------------------------------------
   // RL loops step the same batch with the same pinned buffers every time, so the upload -> kernel -> download sequence is
-  // captured once per (batch, buffers, n) and replayed: one driver call instead of five per chunk.  Measured at 1M
-  // connect_four lanes (profiles/r02_e2e_graph.txt): byte-wide entry 95.7 -> 92.7 us, float entry 468 -> 345 us (its 2-chunk
-  // overlap no longer pays ten driver calls).  Pageable buffers (a captured copy must be a real DMA) and small batches take
-  // the plain stream path below.
+  // captured once per (batch, buffers, n) and replayed: one driver call instead of five per chunk, so the float entry's
+  // 2-chunk overlap no longer pays ten driver calls.  Pageable buffers (a captured copy must be a real DMA) and small
+  // batches take the plain stream path below.
   static bool graphs_broken = false;            // a capture / instantiate failure turns the graph path off for the process
   if (graphs_on && !graphs_broken && n >= (1 << 16)) {
     auto pinned = [](const void* p) {

@@ -73,8 +73,8 @@ __global__ void __launch_bounds__(kBlock, R::kMinBlocks) k_apply(Ctx ctx, typena
 
 // Coalesced store of multi-word legal masks.  A warp owns 32 consecutive lanes, whose mask words are one contiguous range of
 // the output, but written lane by lane (mask[i * W + w] in a loop over w) every store instruction scatters over 32 sectors —
-// for breakthrough (W = 24) that, not the mask arithmetic, was the kernel's limit (ncu, profiles/r02_item9: 2 % of DRAM
-// bandwidth, 15 % SM busy, 40 us for 262k lanes).  The warp stages its 32 x W words in shared memory (row stride odd: no
+// for breakthrough (W = 24) that, not the mask arithmetic, limited the kernel (low DRAM bandwidth and a mostly idle SM
+// under the profiler).  The warp stages its 32 x W words in shared memory (row stride odd: no
 // bank conflicts) and writes the range with fully coalesced 128-byte stores.  Every lane of the warp must call (active =
 // false for lanes past n); W <= MAXW.  `first` = lane index of the warp's lane 0, `n` = lanes in the batch.
 template <int MAXW>

@@ -119,8 +119,8 @@ __global__ void __launch_bounds__(1024) k_cfr(CfrDev d, int iters, int iteration
   // Regret matching of the other player's information states (cfr.cc:693-697 sweeps the whole table) would recompute
   // the same policy from unchanged regrets, so it is skipped.
   // One CTA on purpose: the same kernel as an 8-CTA thread-block cluster (cluster.sync() = barrier.cluster + MEMBAR.GPU +
-  // L1 invalidate per level step, arrays in global memory) was measured at the same 11.2e3 it/s on Leduc and 3x slower
-  // on Kuhn — the level steps are latency-bound, and the cluster barrier costs what the extra threads save.
+  // L1 invalidate per level step, arrays in global memory) was no faster on Leduc and slower on Kuhn — the level steps are
+  // latency-bound, and the cluster barrier costs what the extra threads save.
   const int tid = threadIdx.x, nt = blockDim.x;
   const int L = d.n_levels;
   for (int it = 0; it < iters; ++it) {
@@ -562,9 +562,8 @@ __global__ void __launch_bounds__(kMcLogThreads) k_mccfr_partial_log(int K, int 
 }
 
 // Log -> dense rows: one thread per record slot.  The traversal kernels are latency chains (a few thousand threads walking a
-// tree); letting them also read-modify-write their dense delta rows costs them a third of their time (k_mccfr_es 119 -> 74 us
-// at K = 16,384 on leduc, profiles/r02_item9_summary.md), whereas scattering the same records from a kernel of its own is a
-// few microseconds of fully parallel stores.  Entries are distinct within a traversal and the rows are zero between phases
+// tree); letting them also read-modify-write their dense delta rows lengthens those chains, whereas scattering the same
+// records from a kernel of its own is a few microseconds of fully parallel stores.  Entries are distinct within a traversal and the rows are zero between phases
 // (k_mccfr_apply re-zeroes what it reads), so a plain store reproduces the dense path's cell exactly.
 __global__ void __launch_bounds__(256) k_mccfr_scatter(McLog lg, long long slots, int stride, double* __restrict__ rows) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;

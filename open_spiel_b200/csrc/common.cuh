@@ -1,4 +1,4 @@
-// Shared device/host helpers for the batched game kernels (sm_100a).
+// Shared device/host helpers for the batched game kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,5 +1,5 @@
 // Host definitions of the few device intrinsics the per-game rule cores (rules_*.cuh) and mcts.cuh use, so that the SAME
-// rule-core source the sm_100a kernels are built from also compiles with a plain host compiler (g++ + CUDA's
+// rule-core source the sm_90a kernels are built from also compiles with a plain host compiler (g++ + CUDA's
 // cuda_runtime.h, whose host_defines.h makes __device__ / __forceinline__ harmless).
 // Users: (1) open_spiel_b200/adapter/host_rules.cc — the scalar open_spiel::State adapter (SURVEY §8b: "scalar State
 // methods run the same __host__ __device__ rule core on the CPU"); one State is one object, never a batch: every

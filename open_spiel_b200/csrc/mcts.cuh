@@ -27,8 +27,7 @@
 //
 // Selection is the reference's first-maximum scan in FP64 (an unvisited child is +infinity, so the first unvisited child ends
 // the scan).  A float32 pre-selection with a proven error margin (FP64 only for children whose estimate could still win) was
-// built and measured in round 2: B200's FP64 rate makes it a wash at depth and 10 % slower on shallow trees
-// (profiles/r02_mcts_variants.jsonl), so it was removed.
+// tried and removed.
 // Not implemented: chance nodes in the tree, Dirichlet noise, custom evaluators (the host adapters route those to the
 // stock MCTSBot).
 #pragma once

@@ -144,8 +144,8 @@ struct BreakthroughRules {
     }
   }
 #else
-  // the first version (a loop over the mover's pieces setting bits in an indexed local array), kept for the before / after
-  // measurement under profiles/ (scripts/r02_item9.sh builds a second library with -DB2S_BREAKTHROUGH_LEGAL_LOOP)
+  // the first version (a loop over the mover's pieces setting bits in an indexed local array), kept for before / after
+  // measurements: build a second library with -DB2S_BREAKTHROUGH_LEGAL_LOOP and load it through B2S_LIBRARY
   __device__ static __forceinline__ void legal_nonterminal(const S& s, const Cfg& c, u32* m) {
     for (int i = 0; i < kMaskWords; ++i) m[i] = 0;
     u64 white = s.w & c.board;

@@ -358,9 +358,8 @@ struct GoRules {
   }
   // playout step: try a candidate (an empty non-ko point or pass); false = it was illegal, state untouched.
   // Two restructurings of this step were measured in the MCTS kernel and dropped: (i) replacing the per-chain walks by
-  // two liberty-seeded whole-board floods per move (35 % slower), (ii) one flattened loop over a per-move work list
-  // of chains with early exit on the first liberty (7-35 % slower: 148 registers/thread cost a resident warp per
-  // scheduler).  See profiles/README.md.
+  // two liberty-seeded whole-board floods per move (slower), (ii) one flattened loop over a per-move work list of chains
+  // with early exit on the first liberty (slower: its extra registers cost a resident warp per scheduler).
   __device__ static __forceinline__ bool play_candidate(S& s, int a, const Cfg& c, const Ctx& ctx, long long lane) {
     if (a != c.cells) {
       int r = a / c.n;

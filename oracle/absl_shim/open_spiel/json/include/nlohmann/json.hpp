@@ -1,3 +1,5 @@
-// TEST INFRASTRUCTURE ONLY: forwards to the nlohmann/json 3.11.3 single header that ships inside the image's
-// python environment (the reference expects it at open_spiel/json/, cloned by its install.sh; no network here).
-#include "/opt/prime-rl/.venv/lib/python3.12/site-packages/include/cudnn_frontend/thirdparty/nlohmann/json.hpp"
+// TEST INFRASTRUCTURE ONLY: forwards to an nlohmann/json single header found on the include path (the reference expects
+// it at open_spiel/json/, cloned by its install.sh).  oracle/ref_build.mk and open_spiel_b200/adapter/Makefile add the
+// directory __graft_entry__.json_include_dir() finds as JSON_INC.
+#pragma once
+#include <nlohmann/json.hpp>

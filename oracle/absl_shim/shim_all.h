@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY.  Minimal stand-in for the subset of abseil-cpp (pinned by the reference at tag
-// 20250814.1, open_spiel/scripts/global_variables.sh:33; not vendored, no network here) that the reference
+// 20250814.1, open_spiel/scripts/global_variables.sh:33; not vendored) that the reference
 // files on the hot path include.  It lets oracle/ref_build.mk compile those reference sources UNMODIFIED,
-// where they lie under /root/reference, into oracle/_ref/.  Everything maps onto the C++20 standard library.
+// from the OpenSpiel checkout, into oracle/_ref/.  Everything maps onto the C++20 standard library.
 // Written from the documented abseil API; no abseil source was available or copied.
 //
 // RNG note: absl::uniform_int_distribution / absl::Uniform(int) below restate abseil's published algorithm

@@ -1,11 +1,12 @@
-# TEST INFRASTRUCTURE ONLY.  Compiles the UNMODIFIED reference sources of the hot path, where they lie under
-# /root/reference, against oracle/absl_shim (abseil is not vendored in the reference and cannot be fetched).
-# Outputs go to oracle/_ref/ only (git-ignored, shipped to the GPU box with the snapshot).
-#   make -C oracle -f ref_build.mk            -> _ref/libspiel_ref.a, _ref/ref_bench, _ref/libspiel_ref_c.so
-REF ?= /root/reference
+# TEST INFRASTRUCTURE ONLY.  Compiles the UNMODIFIED reference sources of the hot path, from the OpenSpiel source tree
+# named by REF (default: $OPEN_SPIEL_REFERENCE), against oracle/absl_shim (abseil is not vendored in the reference).
+# Outputs go to oracle/_ref/ only (git-ignored).
+#   make -C oracle -f ref_build.mk REF=<open_spiel checkout>   -> _ref/libspiel_ref.a, _ref/ref_bench, _ref/libspiel_ref_c.so
+REF ?= $(OPEN_SPIEL_REFERENCE)
 CXX := /usr/bin/g++
 # Reference Release flags: open_spiel/CMakeLists.txt:56-61 (-O3 -DNDEBUG); C++20 for the shim's std::span-era library.
-CXXFLAGS := -std=c++20 -O3 -DNDEBUG -fPIC -w -I absl_shim -I $(REF)
+# JSON_INC: a directory holding nlohmann/json.hpp (the reference clones it; __graft_entry__.json_include_dir() finds one)
+CXXFLAGS := -std=c++20 -O3 -DNDEBUG -fPIC -w -I absl_shim -I $(REF) $(if $(JSON_INC),-I $(JSON_INC))
 OS := $(REF)/open_spiel
 SRCS := spiel.cc spiel_utils.cc game_parameters.cc observer.cc policy.cc spiel_bots.cc simultaneous_move_game.cc \
         action_view.cc utils/status.cc utils/usage_logging.cc \

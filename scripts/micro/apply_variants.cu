@@ -1,6 +1,6 @@
 // Microbenchmark (development tool, not part of the library): connect_four ApplyAction kernel variants on
 // rotating 1M-state batches inside a CUDA graph, to pick ILP / block size / launch attributes.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o apply_variants apply_variants.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o apply_variants apply_variants.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -111,9 +111,10 @@ void launch_nowait(ulonglong2* st, const int* act, long long n, unsigned long lo
   cfg.attrs = at; cfg.numAttrs = 1;
   CK(cudaLaunchKernelEx(&cfg, k_apply_nowait<ILP, BLOCK>, st, act, n, err));
 }
+static int g_sms = 0;   // SMs of the device (132 on an H100 SXM), read in main
 template <int ILP, int BLOCK, int BPS>
 void launch_gs(ulonglong2* st, const int* act, long long n, unsigned long long* err, cudaStream_t s) {
-  k_apply_gs<ILP, BLOCK><<<148 * BPS, BLOCK, 0, s>>>(st, act, n, err);
+  k_apply_gs<ILP, BLOCK><<<g_sms * BPS, BLOCK, 0, s>>>(st, act, n, err);
 }
 
 int main(int argc, char** argv) {
@@ -137,6 +138,7 @@ int main(int argc, char** argv) {
     {"gs_ilp4_b256_x4", launch_gs<4, 256, 4>}, {"gs_ilp4_b256_x8", launch_gs<4, 256, 8>}, {"gs_ilp2_b256_x8", launch_gs<2, 256, 8>},
     {"gs_ilp4_b512_x4", launch_gs<4, 512, 4>}, {"gs_ilp1_b256_x8", launch_gs<1, 256, 8>}, {"gs_ilp2_b1024_x2", launch_gs<2, 1024, 2>},
   };
+  CK(cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0));
   cudaStream_t s; CK(cudaStreamCreate(&s));
   cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
   for (auto& v : vs) {

@@ -1,13 +1,14 @@
 #!/usr/bin/env python3
 """Extract golden vectors from the reference's playthrough traces.
 
-Reads /root/reference/open_spiel/integration_tests/playthroughs/<game>.txt (the
+Reads open_spiel/integration_tests/playthroughs/<game>.txt of the OpenSpiel checkout
+__graft_entry__.REFERENCE (the
 line-for-line golden traces checked by the reference's
 integration_tests/playthrough_test.py:73-98; format defined by
 python/algorithms/generate_playthrough.py:211-521) and writes one compact JSON
 fixture per trace under tests/golden/playthroughs/.
 
-Only this script reads /root/reference; the tests read the committed JSON.
+Only this script reads the reference; the tests read the committed JSON.
 
 JSON layout:
   {"game": "<game string>", "header": {"NumDistinctActions": 7, ...},
@@ -27,7 +28,10 @@ import os
 import re
 import sys
 
-REF = "/root/reference/open_spiel/integration_tests/playthroughs"
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+from __graft_entry__ import REFERENCE  # noqa: E402
+
+REF = os.path.join(REFERENCE, "open_spiel", "integration_tests", "playthroughs")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "playthroughs")
 
 TRACES = [

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Generates tests/golden/reference_vectors.json from the UNMODIFIED reference (oracle/_ref, built by oracle/ref_build.mk
-in the container that has /root/reference).  The vectors pin the oracle's algorithm restatements without needing the
+where the reference checkout exists).  The vectors pin the oracle's algorithm restatements without needing the
 reference at test time (tests/test_reference_vectors.py):
   mcts          MCTSBot::MCTSearch root children (action, visits, total reward as hex float) for seeded searches
   mccfr         ExternalSamplingMCCFRSolver tables after N iterations (hex floats)

@@ -3,6 +3,8 @@
 Mirrors the reference's RandomSimTest (tests/basic_tests.cc:321-581): play random games to the end and check
 every observable after every move — here with the oracle supplying the expected values.
 """
+import hashlib
+
 import numpy as np
 import torch
 
@@ -18,10 +20,50 @@ def mask_words_to_lists(words, width):
     return [np.nonzero(row)[0].tolist() for row in bits]
 
 
+def absorb(h, cur, term, legal, rets, obs=None, ist=None):
+    """Feeds what one lane shows at one ply into the sha256 object h: player to move, terminal flag, legal actions,
+    returns (float64, sign of zero included) and, when checked at that ply, the observation / information-state tensor of
+    every player (float32)."""
+    h.update(np.array([int(cur), int(bool(term)), len(legal)] + list(legal), dtype=np.int64).tobytes())
+    h.update(np.asarray(rets, dtype=np.float64).tobytes())
+    for t in (obs or []) + (ist or []):
+        h.update(np.asarray(t, dtype=np.float32).tobytes())
+
+
+def games_digest(hashes):
+    """The digest stored per game in tests/golden/reference_results.json: sha256 over the lanes' sha256 digests in order."""
+    return hashlib.sha256("".join(h.hexdigest() for h in hashes).encode()).hexdigest()
+
+
+def checker_digests(game_string, n_lanes, seed, checker, check_obs_every=3, check_info_state=False):
+    """The games lockstep() plays, on the scalar checker alone (no device): same random actions, same observables fed
+    to absorb() in the same order; returns games_digest().  Used to record the reference's digest."""
+    rng = np.random.RandomState(seed)
+    game = checker(game_string)
+    states = [game.new_initial_state() for _ in range(n_lanes)]
+    hashes = [hashlib.sha256() for _ in range(n_lanes)]
+    P, ply = game.num_players, 0
+    while True:
+        check_obs = check_obs_every and ply % check_obs_every == 0
+        alive = 0
+        for i, st in enumerate(states):
+            ola = st.legal_actions()
+            absorb(hashes[i], st.current_player(), st.is_terminal(), ola, st.returns(),
+                   [st.observation_tensor(p) for p in range(P)] if check_obs else None,
+                   [st.information_state_tensor(p) for p in range(P)] if check_obs and check_info_state else None)
+            if not st.is_terminal():
+                st.apply_action(ola[rng.randint(len(ola))])
+                alive += 1
+        if alive == 0:
+            return games_digest(hashes)
+        ply += 1
+
+
 def lockstep(game_string, n_lanes=512, seed=0, check_obs_every=3, max_plies=None, check_info_state=False,
-             checker=OracleGame):
+             checker=OracleGame, hashes=None):
     """Play n_lanes random games in lock-step on device and on the checker (the oracle restatement, or — passing
-    ref_lib.RefGame — the unmodified reference build); assert equality of everything after every move."""
+    ref_lib.RefGame — the unmodified reference build); assert equality of everything after every move.  hashes: a list
+    of n_lanes sha256 objects that absorb() what each device lane showed (compare with checker_digests())."""
     rng = np.random.RandomState(seed)
     game = b2.load_game(game_string)
     ogame = checker(game_string)
@@ -50,6 +92,9 @@ def lockstep(game_string, n_lanes=512, seed=0, check_obs_every=3, max_plies=None
         actions = np.full(n_lanes, -1, dtype=np.int32)
         alive = 0
         for i, st in enumerate(ostates):
+            if hashes is not None:
+                absorb(hashes[i], cur[i], term[i], legal[i], rets[i], [o[i] for o in obs] if obs is not None else None,
+                       [t[i] for t in ist] if obs is not None and check_info_state else None)
             assert int(cur[i]) == st.current_player(), (game_string, "current_player", i, ply)
             assert bool(term[i]) == st.is_terminal(), (game_string, "is_terminal", i, ply)
             ola = st.legal_actions()

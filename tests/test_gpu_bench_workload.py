@@ -1,8 +1,9 @@
 """Parity of the BENCHED workload itself (SURVEY §8d config 2: "first 1M lanes replayed through the oracle"): the exact
-1,048,576-lane U{0..20}-ply connect_four batch bench.py times (same builder, same seed) is replayed lane by lane on the
-UNMODIFIED reference (oracle/_ref), and every output of the benched step — legal mask before, terminal, current player,
-returns, next legal mask and the full observation tensor after — must match on every lane.  Both host entry points
-(float and compact) are checked on the same batch."""
+1,048,576-lane U{0..20}-ply connect_four batch bench.py times (same builder, same seed) replayed lane by lane on the
+UNMODIFIED reference — live where its build (oracle/_ref) exists, and everywhere through the digests of the reference's
+outputs stored in tests/golden/reference_results.json — and every output of the benched step (legal mask before,
+terminal, current player, returns, next legal mask and the full observation tensor after) must match on every lane.
+Both host entry points (float and compact) are checked on the same batch."""
 import os
 import sys
 
@@ -10,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 
+import golden_lib
 import ref_lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -17,17 +19,19 @@ sys.path.insert(0, ROOT)
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.skipif(not ref_lib.available(), reason="oracle/_ref not built")
 def test_benched_connect_four_batch_equals_reference_on_every_lane():
     import bench
     import open_spiel_b200 as b2
+    gold = golden_lib.reference_results()["bench_workload"]
     n = bench.N_STATES
+    assert gold["n"] == n and gold["seed"] == 0x5EED
     dev = torch.device("cuda", 0)
     game = b2.Game("connect_four", device=0)
     _, snap, actions, hist = bench.build_workload(torch, game, n, dev, seed=0x5EED, with_history=True)
     assert hist.shape == (n, bench.MAX_PREFIX)
-    ref = ref_lib.replay_batch("connect_four", hist.cpu().numpy(), actions.cpu().numpy(), mask_words=1)
-    assert ref["failed_lanes"] == 0
+    hist_np, actions_np = hist.cpu().numpy(), actions.cpu().numpy()
+    assert golden_lib.array_digest(hist_np) == gold["inputs"]["hist"], "the benched inputs differ from the recorded ones"
+    assert golden_lib.array_digest(actions_np) == gold["inputs"]["actions"], "the benched inputs differ from the recorded ones"
     # the device step on the benched batch
     work = game.new_batch(n)
     work.copy_from(snap)
@@ -39,17 +43,24 @@ def test_benched_connect_four_batch_equals_reference_on_every_lane():
     work.check_errors()
     cur, term2, rets2 = work.status()
     obs = work.observation_tensor(player=0)                       # [n, 126] float32
-    assert np.array_equal(mask_before, ref["mask_before"])
-    assert np.array_equal(term.cpu().numpy(), ref["terminal"])
-    assert np.array_equal(term2.cpu().numpy(), ref["terminal"])
-    assert np.array_equal(cur.cpu().numpy(), ref["cur_player"])
-    assert np.array_equal(rets.cpu().numpy(), ref["returns"]) and np.array_equal(rets2.cpu().numpy(), ref["returns"])
-    assert np.array_equal(mask.cpu().numpy().astype(np.uint32), ref["mask_after"])
+    assert torch.equal(term, term2) and torch.equal(rets, rets2)
     F = obs.shape[1]
     pad = torch.zeros((n, (-F) % 32), dtype=obs.dtype, device=dev)
     bits = (torch.cat([obs, pad], dim=1) != 0).reshape(n, -1, 32).to(torch.int64)
     words = (bits << torch.arange(32, device=dev, dtype=torch.int64)).sum(dim=2).cpu().numpy().astype(np.uint32)
-    assert np.array_equal(words, ref["obs_bits"])
+    out = {"mask_before": mask_before, "terminal": term.cpu().numpy().astype(np.uint8),
+           "cur_player": cur.cpu().numpy().astype(np.int8), "returns": rets.cpu().numpy().astype(np.float32),
+           "mask_after": mask.cpu().numpy().astype(np.uint32), "obs_bits": words}
+    assert sorted(out) == sorted(gold["outputs"])
+    if ref_lib.available():
+        live = ref_lib.replay_batch("connect_four", hist_np, actions_np, mask_words=1)
+        assert live["failed_lanes"] == 0
+        for k, v in out.items():
+            assert np.array_equal(v, live[k]), k
+    for k, v in out.items():
+        assert golden_lib.array_digest(v) == gold["outputs"][k], k
+    ref = out                                                     # equal to the reference's outputs, lane for lane
+    assert int(ref["terminal"].sum()) == gold["terminal_lanes"]
     assert int(ref["terminal"].sum()) > 0 and int((ref["terminal"] == 0).sum()) > n // 2      # the step does end some games
     # the two host entry points on the same batch
     work.copy_from(snap)

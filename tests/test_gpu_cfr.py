@@ -1,10 +1,11 @@
-"""GPU parity: device-resident CFR vs the oracle's restatement of algorithms/cfr.cc (and vs the unmodified
-reference when oracle/_ref is present): cumulative regrets, cumulative policy and current policy of every
+"""GPU parity: device-resident CFR vs the oracle's restatement of algorithms/cfr.cc and vs the unmodified reference (live
+when oracle/_ref is present, else its tables and values stored in tests/golden/reference_results.json): cumulative regrets, cumulative policy and current policy of every
 information state, BIT FOR BIT (north-star tolerance is 1e-6), after several iteration counts; tree sizes and
 information-state counts of integration_tests/api_test.py:77-104."""
 import numpy as np
 import pytest
 
+import golden_lib
 import open_spiel_b200 as b2
 import ref_lib
 from oracle_lib import OracleCFR, OracleGame, infostate_tensors
@@ -47,18 +48,22 @@ def test_device_cfr_equals_oracle_bitwise(gs, steps, plus):
         compare(dev.table(), cpu.table(), tensors)
 
 
-@pytest.mark.skipif(not ref_lib.available(), reason="oracle/_ref not shipped")
 @pytest.mark.parametrize("gs,iters", [("kuhn_poker", 300), ("leduc_poker", 25)])
 def test_device_cfr_equals_unmodified_reference(gs, iters):
+    gold = golden_lib.reference_results()["cfr"]["tables"][gs]
+    assert gold["iterations"] == iters
     game = b2.load_game(gs)
     dev = b2.CFRSolver(game)
-    ref = ref_lib.RefCFR(ref_lib.RefGame(gs))
     dev.evaluate_and_update_policy(iters)
-    ref.iterate(iters)
     tensors = infostate_tensors(OracleGame(gs))
-    compare(dev.table(), ref.table(), tensors)
+    assert golden_lib.table_digest(golden_lib.device_table_by_key(dev.table(), tensors)) == gold["table_sha256"]
+    if ref_lib.available():
+        ref = ref_lib.RefCFR(ref_lib.RefGame(gs))
+        ref.iterate(iters)
+        compare(dev.table(), ref.table(), tensors)
     if gs == "kuhn_poker":
-        assert ref.exploitability() <= 0.05          # cfr_test.cc:36-62, now also true of the device tables
+        assert gold["exploitability"] <= 0.05          # cfr_test.cc:36-62, now also true of the device tables
+        assert abs(dev.exploitability() - gold["exploitability"]) <= 1e-9
 
 
 def test_checkpoint_resume_is_exact():
@@ -109,21 +114,24 @@ def test_sharded_traversal_path_is_bit_identical():
         assert np.abs(tr["regrets"]).max() > 0.1       # the tables are not trivially zero
 
 
-@pytest.mark.skipif(not ref_lib.available(), reason="oracle/_ref not shipped")
 @pytest.mark.parametrize("gs,checkpoints", [("kuhn_poker", [1, 10, 100, 300]), ("leduc_poker", [1, 5, 20])])
 def test_device_nash_conv_matches_reference(gs, checkpoints):
     """The evaluation step of the CFR loop (examples/cfr_example.cc:37-46): NashConv / Exploitability of the average
-    policy, device vs the unmodified reference's tabular_exploitability.cc, to 1e-9."""
+    policy, device vs the unmodified reference's tabular_exploitability.cc (live, or its stored values), to 1e-9."""
+    gold = golden_lib.reference_results()["cfr"]["checkpoints"][gs]
+    assert [g["iterations"] for g in gold] == checkpoints
     game = b2.load_game(gs)
     dev = b2.CFRSolver(game)
-    ref = ref_lib.RefCFR(ref_lib.RefGame(gs))
+    ref = ref_lib.RefCFR(ref_lib.RefGame(gs)) if ref_lib.available() else None
     done = 0
-    for it in checkpoints:
+    for it, g in zip(checkpoints, gold):
         dev.evaluate_and_update_policy(it - done)
-        ref.iterate(it - done)
+        if ref is not None:
+            ref.iterate(it - done)
+            assert (ref.nash_conv(), ref.exploitability()) == (g["nash_conv"], g["exploitability"])
         done = it
-        assert abs(dev.nash_conv() - ref.nash_conv()) <= 1e-9, (gs, it)
-        assert abs(dev.exploitability() - ref.exploitability()) <= 1e-9
+        assert abs(dev.nash_conv() - g["nash_conv"]) <= 1e-9, (gs, it)
+        assert abs(dev.exploitability() - g["exploitability"]) <= 1e-9
     if gs == "kuhn_poker":
         assert dev.exploitability() <= 0.05                      # cfr_test.cc:36-62
         assert abs(dev.last_values[2] - (-1.0 / 18.0)) <= 1e-3   # game value for player 0 (cfr_test.cc:40-41)

@@ -201,11 +201,11 @@ def test_device_mcts_matches_reference_mctsbot_in_distribution():
     UNMODIFIED MCTSBot the comparison is statistical: over many independent searches of the same connect_four
     position, the mean share of simulations each root action receives must agree (uct_c = 2, 400 simulations, no
     solver), and so must the mean root value."""
+    import golden_lib
     import ref_lib
-    if not ref_lib.available():
-        pytest.skip("oracle/_ref not shipped")
-    gs, prefix = "connect_four", [3, 3, 2]
-    sims, trees = 400, 512
+    gold = golden_lib.reference_results()["mcts"]
+    gs, prefix = gold["game"], gold["prefix"]
+    sims, trees = gold["sims"], 512
     game = b2.load_game(gs)
     batch = game.new_batch(trees)
     for a in prefix:
@@ -214,19 +214,22 @@ def test_device_mcts_matches_reference_mctsbot_in_distribution():
     v = out["visits"].double()
     dev_share = (v / v.sum(dim=1, keepdim=True)).mean(dim=0).cpu().numpy()
     dev_value = float((out["total_reward"].sum(dim=1) / v.sum(dim=1)).mean())
-    rg = ref_lib.RefGame(gs)
-    st = rg.new_initial_state()
-    for a in prefix:
-        st.apply_action(a)
-    n_ref = 256
-    share = np.zeros(7)
-    value = 0.0
-    for seed in range(n_ref):
-        r = ref_lib.ref_mcts(rg, st, 2.0, sims, 1, False, seed + 1)
-        tot = sum(vv for _, vv, _ in r["children"])
-        for a, vv, _ in r["children"]:
-            share[a] += vv / tot / n_ref
-        value += sum(rw for _, _, rw in r["children"]) / tot / n_ref
+    share, value = np.array(gold["share"]), gold["value"]       # the reference's 256 searches (stored)
+    if ref_lib.available():                                      # and live, where the reference build exists
+        rg = ref_lib.RefGame(gs)
+        st = rg.new_initial_state()
+        for a in prefix:
+            st.apply_action(a)
+        n_ref = gold["n_ref"]
+        share = np.zeros(7)
+        value = 0.0
+        for seed in range(n_ref):
+            r = ref_lib.ref_mcts(rg, st, 2.0, sims, 1, False, seed + 1)
+            tot = sum(vv for _, vv, _ in r["children"])
+            for a, vv, _ in r["children"]:
+                share[a] += vv / tot / n_ref
+            value += sum(rw for _, _, rw in r["children"]) / tot / n_ref
+        assert np.array_equal(share, np.array(gold["share"])) and value == gold["value"]
     # standard error of a mean share over a few hundred searches is ~0.005; allow 0.03
     assert np.abs(dev_share - share).max() < 0.03, (dev_share, share)
     assert abs(dev_value - value) < 0.05, (dev_value, value)

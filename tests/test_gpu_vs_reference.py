@@ -1,13 +1,17 @@
-"""GPU parity directly against the UNMODIFIED reference (oracle/_ref/libspiel_ref_c.so, shipped with the snapshot):
-the same lock-step harness as test_gpu_parity_games.py with the real open_spiel::State objects as the checker.
+"""GPU parity directly against the UNMODIFIED reference: the same lock-step harness as test_gpu_parity_games.py, with the
+real open_spiel::State objects as the checker where the reference build (oracle/_ref/libspiel_ref_c.so) exists, and
+everywhere against the per-lane digests of the reference's games stored in tests/golden/reference_results.json.
 Also: size-independent properties at full batch sizes, and ragged / empty batches."""
+import hashlib
+
 import numpy as np
 import pytest
 import torch
 
+import golden_lib
 import open_spiel_b200 as b2
 import ref_lib
-from parity import lockstep
+from parity import games_digest, lockstep
 
 pytestmark = pytest.mark.gpu
 
@@ -16,12 +20,15 @@ GAMES = [("tic_tac_toe", 128), ("connect_four", 128), ("breakthrough", 64), ("he
          ("mnk", 16), ("mnk(m=5,n=4,k=3)", 64), ("othello", 64), ("y(board_size=9)", 64), ("havannah(board_size=4,swap=True)", 64), ("havannah", 16)]
 
 
-@pytest.mark.skipif(not ref_lib.available(), reason="oracle/_ref not shipped")
 @pytest.mark.parametrize("gs,lanes", GAMES, ids=[g for g, _ in GAMES])
 def test_device_equals_unmodified_reference(gs, lanes):
-    steps = lockstep(gs, n_lanes=lanes, seed=99, checker=ref_lib.RefGame,
-                     check_info_state=gs in ("kuhn_poker", "leduc_poker"))
+    gold = golden_lib.reference_results()["lockstep"]
+    hashes = [hashlib.sha256() for _ in range(lanes)]
+    checker = ref_lib.RefGame if ref_lib.available() else None
+    steps = lockstep(gs, n_lanes=lanes, seed=gold["seed"], hashes=hashes, check_info_state=gs in ("kuhn_poker", "leduc_poker"),
+                     **({"checker": checker} if checker else {}))
     assert steps > lanes
+    assert games_digest(hashes) == gold["digests"][gs], (gs, "the device's games differ from the reference's")
 
 
 @pytest.mark.parametrize("gs,n", [("go(board_size=9)", 1 << 17), ("hex", 1 << 18), ("breakthrough", 1 << 20),

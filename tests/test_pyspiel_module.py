@@ -18,10 +18,11 @@ if not glob.glob(os.path.join(BUILD, "pyspiel*.so")):
 sys.path.insert(0, BUILD)
 import pyspiel  # noqa: E402
 
+from __graft_entry__ import REFERENCE  # noqa: E402
 from open_spiel_b200 import playthrough as pt  # noqa: E402
 
 HASHES = json.load(open(os.path.join(ROOT, "tests", "golden", "playthrough_sha256.json")))
-REF_DIR = "/root/reference/open_spiel/integration_tests/playthroughs"
+REF_DIR = os.path.join(REFERENCE, "open_spiel", "integration_tests", "playthroughs")
 
 
 @pytest.mark.parametrize("name", sorted(HASHES))
@@ -31,7 +32,7 @@ def test_reference_playthrough_regenerates_byte_identically(name):
     assert len(text.encode("utf-8")) == rec["bytes"]
     assert hashlib.sha256(text.encode("utf-8")).hexdigest() == rec["sha256"]
     ref = os.path.join(REF_DIR, name + ".txt")
-    if os.path.exists(ref):                      # in the build container: the reference's own replay() comparison
+    if os.path.exists(ref):                      # where the reference checkout exists: its own replay() comparison
         original = open(ref, encoding="utf-8").read()
         assert pt.replay(original, pyspiel) == original
 

@@ -1,6 +1,6 @@
-"""Pins the oracle restatement against the UNMODIFIED reference (oracle/_ref, built from /root/reference by
+"""Pins the oracle restatement against the UNMODIFIED reference (oracle/_ref, built from the OpenSpiel checkout by
 oracle/ref_build.mk with the abseil shim): random playouts, every observable compared after every move.
-Skipped when oracle/_ref has not been built (it is built by __graft_entry__.build() when /root/reference exists)."""
+Skipped when oracle/_ref has not been built (it is built by __graft_entry__.build() when that checkout exists)."""
 import numpy as np
 import pytest
 
