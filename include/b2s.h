@@ -81,7 +81,8 @@ typedef struct b2s_game_info {
   int32_t observation_tensor_size;
   int32_t information_state_tensor_size;   /* 0 when the game provides none */
   int32_t mask_words;                      /* ceil(max(num_distinct_actions, max_chance_outcomes)/32) */
-  int32_t state_bytes;                     /* bytes of packed state per lane (excluding history) */
+  int32_t state_bytes;                     /* bytes of a lane's packed state blob, b2s_state_get / _set (excluding history;
+                                              a batch may hold the lane in fewer: connect_four keeps 8) */
   int32_t history_bytes;                   /* extra per-lane bytes (go: superko hash history) */
   double min_utility, max_utility;
   int32_t obs_shape[4];                    /* ObservationTensorShape, zero padded */

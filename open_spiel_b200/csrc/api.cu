@@ -498,20 +498,24 @@ int b2s_error_count(void* batch, int64_t* count, int64_t* first_bad_lane, void* 
   return 0;
 }
 
-// Packed lane blob: the kChunks chunks in plane order, then (go) the history column.
+// Packed lane blob: the kChunks chunks in plane order (decoded from the batch's R::Packed where a rule core has one), then
+// (go) the history column.
 int b2s_state_get(void* batch, int64_t idx, void* host_blob, size_t cap) {
   if (int r = check(batch, 0)) return r;
   Batch* B = (Batch*)batch;
   if (idx < 0 || idx >= B->cap) return fail("lane out of range");
-  size_t cb = B->ops->chunk_bytes();
-  size_t need = cb * B->ops->chunks() + B->info.history_bytes;
+  size_t cb = B->ops->chunk_bytes(), sb = (size_t)B->info.state_bytes;
+  size_t need = sb + B->info.history_bytes;
   if (cap < need) return fail("blob too small");
   CU(cudaDeviceSynchronize());
-  char* out = (char*)host_blob;
+  std::vector<uint4> stored((cb * B->ops->chunks() + 15) / 16), blob((sb + 15) / 16);
   for (int k = 0; k < B->ops->chunks(); ++k)
-    CU(cudaMemcpy(out + k * cb, (char*)B->planes + ((size_t)k * B->cap + idx) * cb, cb, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy((char*)stored.data() + k * cb, (char*)B->planes + ((size_t)k * B->cap + idx) * cb, cb, cudaMemcpyDeviceToHost));
+  B->ops->stored_to_blob(stored.data(), blob.data());
+  char* out = (char*)host_blob;
+  memcpy(out, blob.data(), sb);
   if (B->info.history_bytes)
-    CU(cudaMemcpy2D(out + cb * B->ops->chunks(), sizeof(u64), B->hist + idx, sizeof(u64) * B->cap, sizeof(u64),
+    CU(cudaMemcpy2D(out + sb, sizeof(u64), B->hist + idx, sizeof(u64) * B->cap, sizeof(u64),
                     B->info.history_bytes / sizeof(u64), cudaMemcpyDeviceToHost));
   return 0;
 }
@@ -519,15 +523,18 @@ int b2s_state_set(void* batch, int64_t idx, const void* host_blob, size_t len) {
   if (int r = check(batch, 0)) return r;
   Batch* B = (Batch*)batch;
   if (idx < 0 || idx >= B->cap) return fail("lane out of range");
-  size_t cb = B->ops->chunk_bytes();
-  size_t need = cb * B->ops->chunks() + B->info.history_bytes;
+  size_t cb = B->ops->chunk_bytes(), sb = (size_t)B->info.state_bytes;
+  size_t need = sb + B->info.history_bytes;
   if (len != need) return fail("blob size mismatch");
   CU(cudaDeviceSynchronize());
   const char* in = (const char*)host_blob;
+  std::vector<uint4> stored((cb * B->ops->chunks() + 15) / 16), blob((sb + 15) / 16);
+  memcpy(blob.data(), in, sb);
+  B->ops->blob_to_stored(blob.data(), stored.data());
   for (int k = 0; k < B->ops->chunks(); ++k)
-    CU(cudaMemcpy((char*)B->planes + ((size_t)k * B->cap + idx) * cb, in + k * cb, cb, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy((char*)B->planes + ((size_t)k * B->cap + idx) * cb, (const char*)stored.data() + k * cb, cb, cudaMemcpyHostToDevice));
   if (B->info.history_bytes)
-    CU(cudaMemcpy2D(B->hist + idx, sizeof(u64) * B->cap, in + cb * B->ops->chunks(), sizeof(u64), sizeof(u64),
+    CU(cudaMemcpy2D(B->hist + idx, sizeof(u64) * B->cap, in + sb, sizeof(u64), sizeof(u64),
                     B->info.history_bytes / sizeof(u64), cudaMemcpyHostToDevice));
   return 0;
 }
@@ -619,18 +626,19 @@ int b2s_mcts_search(void* roots_batch, int64_t n_trees, const b2s_mcts_config* c
   if (n_trees == 0) return 0;
   Batch* B = (Batch*)roots_batch;
   cudaStream_t st = (cudaStream_t)stream;
-  // scratch lanes: same layout as the roots; only the per-lane history column (go) is ever written
+  // scratch lanes: the roots in the lane-blob form (state_bytes per lane) the search reads them in; only the per-lane
+  // history column (go) is ever written
   if (B->mcts_work_cap < n_trees) {
     if (B->mcts_work) cudaFree(B->mcts_work);
     if (B->mcts_hist) cudaFree(B->mcts_hist);
     B->mcts_work = nullptr; B->mcts_hist = nullptr; B->mcts_work_cap = 0;
-    CU(cudaMalloc(&B->mcts_work, B->ops->chunk_bytes() * (size_t)B->ops->chunks() * (size_t)n_trees));
+    CU(cudaMalloc(&B->mcts_work, (size_t)B->info.state_bytes * (size_t)n_trees));
     if (B->info.history_bytes) CU(cudaMalloc((void**)&B->mcts_hist, (size_t)B->info.history_bytes * (size_t)n_trees));
     B->mcts_work_cap = n_trees;
   }
   Ctx work;
   work.planes = B->mcts_work; work.cap = B->mcts_work_cap; work.hist = B->mcts_hist; work.err = B->err;
-  B->ops->copy(work, 0, B->ctx(), 0, n_trees, st);
+  B->ops->copy_to_blob(work, B->ctx(), n_trees, st);
   // log table filled by the host's std::log
   int need = cfg->max_simulations + 2;
   if (B->mcts_log_n < need) {
@@ -686,7 +694,7 @@ int b2s_mcts_search(void* roots_batch, int64_t n_trees, const b2s_mcts_config* c
   { const char* t = getenv("B2S_MCTS_TUNING"); a.tuning = t ? atoi(t) : 0; }
   a.visits_out = visit_counts_d; a.reward_out = total_reward_d; a.outcome_out = outcome_p0_d;
   a.best_out = best_action_d; a.sims_out = sims_run_d; a.gc_out = cfg->gc_runs_d; a.err = B->err;
-  const char* e = B->ops->mcts(B->ctx(), work, n_trees, a, st);
+  const char* e = B->ops->mcts(work, work, n_trees, a, st);
   if (e) return fail(e);
   if (int r = post()) return r;
   CU(cudaStreamSynchronize(st));          // the search is a long-running call; results are ready on return

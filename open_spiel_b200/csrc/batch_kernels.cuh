@@ -3,6 +3,7 @@
 // integer ops, coalesced stores.  Grid = ceil(n / block); blocks of 256 threads.
 #pragma once
 #include <new>
+#include <string.h>
 
 #include "common.cuh"
 
@@ -43,31 +44,33 @@ __global__ void __launch_bounds__(kBlock) k_reset(Ctx ctx, typename R::Cfg cfg, 
   if (i >= n) return;
   typename R::S s;
   R::init(s, cfg, ctx, i);
-  R::store(s, ctx, i);
+  store_state<R>(s, cfg, ctx, i);
 }
 
 // State::ApplyAction over the batch (spiel.cc:441-451).  Each thread owns ILP lanes, block-strided so every
 // access stays coalesced; all loads (action + packed state) are issued before any compute so that a thread
-// has ILP independent 128-bit requests in flight (the kernel is a pure HBM stream).
+// has ILP independent requests in flight (the kernel is a pure HBM stream).
 template <class R, int ILP>
 __global__ void __launch_bounds__(kBlock, R::kMinBlocks) k_apply(Ctx ctx, typename R::Cfg cfg, const int* __restrict__ actions, long long n) {
   pdl_wait();
   long long base = (long long)blockIdx.x * (kBlock * ILP) + threadIdx.x;
   int a[ILP];
-  typename R::S s[ILP];
+  Fetched<R> pk[ILP];
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
     a[j] = -1;
-    if (i < n) { a[j] = __ldg(actions + i); R::load(s[j], ctx, i); }
+    if (i < n) { a[j] = __ldg(actions + i); fetch_state<R>(pk[j], ctx, i); }
   }
   pdl_launch_dependents();
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
     if (a[j] == -1) continue;
-    if (R::terminal(s[j], cfg) || !R::apply(s[j], a[j], cfg, ctx, i)) { flag_error(ctx.err, ctx.lane0 + i); continue; }
-    R::store(s[j], ctx, i);
+    typename R::S s;
+    unpack_state<R>(s, pk[j], cfg);
+    if (R::terminal(s, cfg) || !R::apply(s, a[j], cfg, ctx, i)) { flag_error(ctx.err, ctx.lane0 + i); continue; }
+    store_state<R>(s, cfg, ctx, i);
   }
 }
 
@@ -108,18 +111,22 @@ __device__ __forceinline__ void store_masks_coalesced(u32* __restrict__ mask, lo
 template <class R, int ILP>
 __global__ void __launch_bounds__(kBlock) k_legal_mask(Ctx ctx, typename R::Cfg cfg, u32* __restrict__ mask, int mask_words, long long n) {
   long long base = (long long)blockIdx.x * (kBlock * ILP) + threadIdx.x;
-  typename R::S s[ILP];
+  Fetched<R> pk[ILP];
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
-    if (i < n) R::load(s[j], ctx, i);
+    if (i < n) fetch_state<R>(pk[j], ctx, i);
   }
   __shared__ MaskStage<R::kMaskWords == 1 ? 0 : R::kMaskWords> stage;
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
     u32 m[R::kMaskWords];
-    if (i < n) R::legal(s[j], cfg, m);
+    if (i < n) {
+      typename R::S s;
+      unpack_state<R>(s, pk[j], cfg);
+      R::legal(s, cfg, m);
+    }
     if (R::kMaskWords == 1) {
       if (i < n) mask[i] = m[0];
     } else {
@@ -133,7 +140,7 @@ __global__ void __launch_bounds__(kBlock) k_legal_list(Ctx ctx, typename R::Cfg 
   long long i = (long long)blockIdx.x * kBlock + threadIdx.x;
   if (i >= n) return;
   typename R::S s;
-  R::load(s, ctx, i);
+  load_state<R>(s, cfg, ctx, i);
   u32 m[R::kMaskWords];
   R::legal(s, cfg, m);
   int k = 0;
@@ -152,22 +159,24 @@ __global__ void __launch_bounds__(kBlock) k_legal_list(Ctx ctx, typename R::Cfg 
 template <class R, int ILP>
 __global__ void __launch_bounds__(kBlock) k_status(Ctx ctx, typename R::Cfg cfg, signed char* __restrict__ cur, unsigned char* __restrict__ term, float* __restrict__ rets, long long n) {
   long long base = (long long)blockIdx.x * (kBlock * ILP) + threadIdx.x;
-  typename R::S s[ILP];
+  Fetched<R> pk[ILP];
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
-    if (i < n) R::load(s[j], ctx, i);
+    if (i < n) fetch_state<R>(pk[j], ctx, i);
   }
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
     if (i >= n) continue;
-    int cp = R::cur_player(s[j], cfg);
+    typename R::S s;
+    unpack_state<R>(s, pk[j], cfg);
+    int cp = R::cur_player(s, cfg);
     if (cur) cur[i] = (signed char)cp;
     if (term) term[i] = cp == kTerminalPlayerId ? 1 : 0;
     if (rets) {
       float r[R::kPlayers];
-      R::returns(s[j], cfg, r);
+      R::returns(s, cfg, r);
       if (R::kPlayers == 2) reinterpret_cast<float2*>(rets)[i] = make_float2(r[0], r[1]);
       else { const int np = rule_num_players<R>(cfg); for (int p = 0; p < np; ++p) rets[i * np + p] = r[p]; }
     }
@@ -180,12 +189,12 @@ __global__ void __launch_bounds__(kBlock) k_step_fused(Ctx ctx, typename R::Cfg 
   pdl_wait();
   long long base = (long long)blockIdx.x * (kBlock * ILP) + threadIdx.x;
   int a[ILP];
-  typename R::S s[ILP];
+  Fetched<R> pk[ILP];
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
     a[j] = -1;
-    if (i < n) { a[j] = __ldg(actions + i); R::load(s[j], ctx, i); }
+    if (i < n) { a[j] = __ldg(actions + i); fetch_state<R>(pk[j], ctx, i); }
   }
   pdl_launch_dependents();
   __shared__ MaskStage<R::kMaskWords == 1 ? 0 : R::kMaskWords> stage;
@@ -195,21 +204,23 @@ __global__ void __launch_bounds__(kBlock) k_step_fused(Ctx ctx, typename R::Cfg 
     const bool live = i < n;
     u32 m[R::kMaskWords];
     if (live) {
+      typename R::S s;
+      unpack_state<R>(s, pk[j], cfg);
       if (a[j] != -1) {
-        if (R::terminal(s[j], cfg) || !R::apply(s[j], a[j], cfg, ctx, i)) flag_error(ctx.err, ctx.lane0 + i);
-        else R::store(s[j], ctx, i);
+        if (R::terminal(s, cfg) || !R::apply(s, a[j], cfg, ctx, i)) flag_error(ctx.err, ctx.lane0 + i);
+        else store_state<R>(s, cfg, ctx, i);
       }
-      bool t = R::terminal(s[j], cfg);
+      bool t = R::terminal(s, cfg);
       if (term) term[i] = t ? 1 : 0;
       if (rets) {
         float r[R::kPlayers];
-        R::returns(s[j], cfg, r);
+        R::returns(s, cfg, r);
         if (R::kPlayers == 2) reinterpret_cast<float2*>(rets)[i] = make_float2(r[0], r[1]);
         else { const int np = rule_num_players<R>(cfg); for (int p = 0; p < np; ++p) rets[i * np + p] = r[p]; }
       }
       if (mask) {
         if (t) { for (int w = 0; w < R::kMaskWords; ++w) m[w] = 0; }
-        else R::legal_nonterminal(s[j], cfg, m);
+        else R::legal_nonterminal(s, cfg, m);
       }
     }
     if (mask) {                                            // uniform over the grid
@@ -232,7 +243,7 @@ __global__ void __launch_bounds__(kBlock) k_step_compact(Ctx ctx, typename R::Cf
   pdl_wait();
   long long base = (long long)blockIdx.x * (kBlock * ILP) + threadIdx.x;
   int a[ILP];
-  typename R::S s[ILP];
+  Fetched<R> pk[ILP];
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
@@ -240,7 +251,7 @@ __global__ void __launch_bounds__(kBlock) k_step_compact(Ctx ctx, typename R::Cf
     if (i < n) {
       AT raw = __ldg(actions + i);
       a[j] = (sizeof(AT) == 1 && (unsigned char)raw == 0xFFu) ? -1 : (int)raw;
-      R::load(s[j], ctx, i);
+      fetch_state<R>(pk[j], ctx, i);
     }
   }
   pdl_launch_dependents();
@@ -251,19 +262,21 @@ __global__ void __launch_bounds__(kBlock) k_step_compact(Ctx ctx, typename R::Cf
     const bool live = i < n;
     u32 m[R::kMaskWords];
     if (live) {
+      typename R::S s;
+      unpack_state<R>(s, pk[j], cfg);
       if (a[j] != -1) {
-        if (R::terminal(s[j], cfg) || !R::apply(s[j], a[j], cfg, ctx, i)) flag_error(ctx.err, ctx.lane0 + i);
-        else R::store(s[j], ctx, i);
+        if (R::terminal(s, cfg) || !R::apply(s, a[j], cfg, ctx, i)) flag_error(ctx.err, ctx.lane0 + i);
+        else store_state<R>(s, cfg, ctx, i);
       }
-      bool t = R::terminal(s[j], cfg);
+      bool t = R::terminal(s, cfg);
       unsigned st = 0;
       if (t) {
         float r[R::kPlayers];
-        R::returns(s[j], cfg, r);
+        R::returns(s, cfg, r);
         st = 0x80u | (r[0] > 0.f ? 1u : (r[0] < 0.f ? 2u : 0u));
         for (int w = 0; w < R::kMaskWords; ++w) m[w] = 0;
       } else if (small_mask || mask) {
-        R::legal_nonterminal(s[j], cfg, m);
+        R::legal_nonterminal(s, cfg, m);
         if (small_mask) st = m[0] & 0x7Fu;
       }
       status[i] = (unsigned char)st;
@@ -290,7 +303,7 @@ __global__ void __launch_bounds__(kBlock) k_obs(Ctx ctx, typename R::Cfg cfg, in
   int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (i < n) {
     typename R::S s;
-    R::load(s, ctx, i);
+    load_state<R>(s, cfg, ctx, i);
     if (zero_terminal) dead_flags[threadIdx.x] = R::terminal(s, cfg) ? 1 : 0;
     int pl = player;
     if (pl < 0) { pl = R::cur_player(s, cfg); if (pl < 0) pl = 0; }
@@ -349,14 +362,14 @@ __global__ void __launch_bounds__(kBlock) k_rollout(Ctx ctx, typename R::Cfg cfg
   long long i = (long long)blockIdx.x * kBlock + threadIdx.x;
   if (i >= n) return;
   typename R::S s;
-  R::load(s, ctx, i);
+  load_state<R>(s, cfg, ctx, i);
   int ply = 0;
   while (!R::terminal(s, cfg) && ply < max_plies) {
     auto draw = [&](u32 b, u32 n) { return philox_uniform(seed, (u64)(i + lane_offset), b, n); };
     playout_step<R>(s, cfg, ctx, i, mask_words, draw, (u32)ply);
     ++ply;
   }
-  R::store(s, ctx, i);
+  store_state<R>(s, cfg, ctx, i);
   if (plies) plies[i] = ply;
   if (rets) {
     float r[R::kPlayers];
@@ -394,10 +407,10 @@ __global__ void __launch_bounds__(kBlock) k_traj_begin(Ctx ctx, typename R::Cfg 
   if (i >= n) return;
   if (lengths) lengths[i] = 0;
   typename R::S s;
-  R::load(s, ctx, i);
+  load_state<R>(s, cfg, ctx, i);
   if (R::cur_player(s, cfg) != kChancePlayerId) return;
   traj_resolve_chance<R>(s, cfg, ctx, i, seed, (u64)(i + lane_offset), mask_words, 0u);
-  R::store(s, ctx, i);
+  store_state<R>(s, cfg, ctx, i);
 }
 
 // Zero-copy form of k_step_compact for pinned, device-mapped host buffers (b2s_step_fused_host_compact): the kernel reads the
@@ -421,30 +434,32 @@ __global__ void __launch_bounds__(kBlock) k_step_compact_zc(Ctx ctx, typename R:
     else for (int k = vec; k < here; ++k) act_s[k] = actions[b0 + k];
   }
   long long base = b0 + threadIdx.x;
-  typename R::S s[ILP];
+  Fetched<R> pk[ILP];
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
-    if (i < n) R::load(s[j], ctx, i);
+    if (i < n) fetch_state<R>(pk[j], ctx, i);
   }
   __syncthreads();
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
     if (i >= n) continue;
+    typename R::S s;
+    unpack_state<R>(s, pk[j], cfg);
     const unsigned raw = act_s[threadIdx.x + j * kBlock];
     if (raw != 0xFFu) {
-      if (R::terminal(s[j], cfg) || !R::apply(s[j], (int)raw, cfg, ctx, i)) flag_error(ctx.err, ctx.lane0 + i);
-      else R::store(s[j], ctx, i);
+      if (R::terminal(s, cfg) || !R::apply(s, (int)raw, cfg, ctx, i)) flag_error(ctx.err, ctx.lane0 + i);
+      else store_state<R>(s, cfg, ctx, i);
     }
     unsigned st = 0;
-    if (R::terminal(s[j], cfg)) {
+    if (R::terminal(s, cfg)) {
       float r[R::kPlayers];
-      R::returns(s[j], cfg, r);
+      R::returns(s, cfg, r);
       st = 0x80u | (r[0] > 0.f ? 1u : (r[0] < 0.f ? 2u : 0u));
     } else if (small_mask) {
       u32 m[R::kMaskWords];
-      R::legal_nonterminal(s[j], cfg, m);
+      R::legal_nonterminal(s, cfg, m);
       st = m[0] & 0x7Fu;
     }
     st_s[threadIdx.x + j * kBlock] = (unsigned char)st;
@@ -475,7 +490,7 @@ __global__ void __launch_bounds__(kBlock) k_traj_step(Ctx ctx, typename R::Cfg c
   int a = 0, pl = 0;
   unsigned char valid = 0, nit = 0;
   if (live) {
-    R::load(s, ctx, i);
+    load_state<R>(s, cfg, ctx, i);
     if (R::terminal(s, cfg)) {
       // padding as BatchedTrajectory::ResizeFields (trajectories.cc:62-96): legal mask all ones, everything else 0
       for (int w = 0; w < R::kMaskWords; ++w) {
@@ -494,7 +509,7 @@ __global__ void __launch_bounds__(kBlock) k_traj_step(Ctx ctx, typename R::Cfg c
       apply_known_legal<R>(s, a, cfg, ctx, i);
       traj_resolve_chance<R>(s, cfg, ctx, i, seed, g, mask_words, b0);
       nit = R::terminal(s, cfg) ? 1 : 0;
-      R::store(s, ctx, i);
+      store_state<R>(s, cfg, ctx, i);
       if (nit && o.lengths) o.lengths[i] = t + 1;
     }
   }
@@ -516,7 +531,7 @@ __global__ void __launch_bounds__(kBlock) k_traj_finish(Ctx ctx, typename R::Cfg
   long long i = (long long)blockIdx.x * kBlock + threadIdx.x;
   if (i >= n) return;
   typename R::S s;
-  R::load(s, ctx, i);
+  load_state<R>(s, cfg, ctx, i);
   if (!R::terminal(s, cfg)) flag_error(ctx.err, i);
   if (rewards) {
     float r[R::kPlayers];
@@ -532,8 +547,8 @@ __global__ void __launch_bounds__(kBlock) k_broadcast(Ctx dst, long long dst0, l
   long long i = (long long)blockIdx.x * kBlock + threadIdx.x;
   if (i >= count) return;
   typename R::S s;
-  R::load(s, srcctx, src);
-  R::store(s, dst, dst0 + i);
+  load_state<R>(s, cfg, srcctx, src);
+  store_state<R>(s, cfg, dst, dst0 + i);
   R::copy_history(dst, dst0 + i, srcctx, src, s, cfg);
 }
 
@@ -543,9 +558,21 @@ __global__ void __launch_bounds__(kBlock) k_copy(Ctx dst, long long dst0, Ctx sr
   long long i = (long long)blockIdx.x * kBlock + threadIdx.x;
   if (i >= count) return;
   typename R::S s;
-  R::load(s, srcctx, src0 + i);
-  R::store(s, dst, dst0 + i);
+  load_state<R>(s, cfg, srcctx, src0 + i);
+  store_state<R>(s, cfg, dst, dst0 + i);
   R::copy_history(dst, dst0 + i, srcctx, src0 + i, s, cfg);
+}
+
+// Clone lanes [0, count) into the lane-blob form (R::store, as b2s_state_get returns a lane): the MCTS kernel reads its roots
+// so, as does the host emulation of it.
+template <class R>
+__global__ void __launch_bounds__(kBlock) k_copy_to_blob(Ctx dst, Ctx srcctx, long long count, typename R::Cfg cfg) {
+  long long i = (long long)blockIdx.x * kBlock + threadIdx.x;
+  if (i >= count) return;
+  typename R::S s;
+  load_state<R>(s, cfg, srcctx, i);
+  R::store(s, dst, i);
+  R::copy_history(dst, i, srcctx, i, s, cfg);
 }
 
 // Gather-clone: dst[i] = src[src_lanes[i]] (tree expansion: one child lane per (parent, action) pair).
@@ -556,8 +583,8 @@ __global__ void __launch_bounds__(kBlock) k_gather(Ctx dst, Ctx srcctx, const lo
   long long sl = src_lanes[i];
   if (sl < 0 || sl >= srcctx.cap) { flag_error(dst.err, i); return; }
   typename R::S s;
-  R::load(s, srcctx, sl);
-  R::store(s, dst, i);
+  load_state<R>(s, cfg, srcctx, sl);
+  store_state<R>(s, cfg, dst, i);
   R::copy_history(dst, i, srcctx, sl, s, cfg);
 }
 
@@ -573,8 +600,11 @@ struct GameOps {
   virtual ~GameOps() {}
   virtual void device_init() = 0;     // called with the batch's device current
   virtual const char* configure(const b2s_params& p, b2s_game_info& gi) = 0;
-  virtual size_t chunk_bytes() const = 0;
+  virtual size_t chunk_bytes() const = 0;   // one chunk of a lane as the batch holds it (StoredChunk)
   virtual int chunks() const = 0;
+  // b2s_state_get / b2s_state_set: a lane's stored chunks (plane order, 16-byte aligned) <-> its blob (state_bytes, aligned)
+  virtual void stored_to_blob(const void* stored, void* blob) const = 0;
+  virtual void blob_to_stored(const void* blob, void* stored) const = 0;
   virtual void reset(const Ctx&, long long n, cudaStream_t) = 0;
   virtual void apply(const Ctx&, const int* a, long long n, cudaStream_t) = 0;
   virtual void legal_mask(const Ctx&, u32* m, long long n, cudaStream_t) = 0;
@@ -588,6 +618,7 @@ struct GameOps {
   virtual void rollout(const Ctx&, u64 seed, long long lane_offset, float* rets, int* plies, long long n, cudaStream_t) = 0;
   virtual void broadcast(const Ctx& dst, long long dst0, long long count, const Ctx& src, long long srclane, cudaStream_t) = 0;
   virtual void copy(const Ctx& dst, long long dst0, const Ctx& src, long long src0, long long count, cudaStream_t) = 0;
+  virtual void copy_to_blob(const Ctx& dst, const Ctx& src, long long count, cudaStream_t) = 0;   // dst in the lane-blob form
   virtual void gather(const Ctx& dst, const Ctx& src, const long long* src_lanes, long long count, cudaStream_t) = 0;
   virtual void traj_begin(const Ctx&, u64 seed, long long lane_offset, int* lengths, long long n, cudaStream_t) = 0;
   virtual void traj_step(const Ctx&, u64 seed, long long lane_offset, int t, const TrajStepOut& o, long long n, cudaStream_t) = 0;
@@ -596,6 +627,28 @@ struct GameOps {
   virtual const char* mcts(const Ctx& roots, const Ctx& work, long long n, const struct MctsArgs& args, cudaStream_t) = 0;
   b2s_game_info info;
 };
+
+// A lane's blob is its stored chunks, or for a rule core with R::Packed the decoded state written by R::store.
+template <class R, class Q = typename R::Packed>
+void stored_to_blob_impl(const typename R::Cfg& c, const void* stored, void* blob, int) {
+  typename R::S s;
+  R::unpack(s, *static_cast<const Q*>(stored), c);
+  Ctx b = {};
+  b.planes = blob; b.cap = 1;
+  R::store(s, b, 0);
+}
+template <class R>
+void stored_to_blob_impl(const typename R::Cfg&, const void* stored, void* blob, long) { memcpy(blob, stored, sizeof(typename R::Chunk) * R::kChunks); }
+template <class R, class Q = typename R::Packed>
+void blob_to_stored_impl(const typename R::Cfg& c, const void* blob, void* stored, int) {
+  typename R::S s;
+  Ctx b = {};
+  b.planes = const_cast<void*>(blob); b.cap = 1;
+  R::load(s, b, 0);
+  *static_cast<Q*>(stored) = R::pack(s, c);
+}
+template <class R>
+void blob_to_stored_impl(const typename R::Cfg&, const void* blob, void* stored, long) { memcpy(stored, blob, sizeof(typename R::Chunk) * R::kChunks); }
 
 inline unsigned grid_for(long long n, int ilp = 1) { return (unsigned)((n + (long long)kBlock * ilp - 1) / ((long long)kBlock * ilp)); }
 
@@ -624,7 +677,9 @@ struct GameOpsT : GameOps {
     return nullptr;
   }
   void device_init() override { call_device_init<R>(0); }
-  size_t chunk_bytes() const override { return sizeof(typename R::Chunk); }
+  size_t chunk_bytes() const override { return sizeof(StoredChunk<R>); }
+  void stored_to_blob(const void* stored, void* blob) const override { stored_to_blob_impl<R>(cfg, stored, blob, 0); }
+  void blob_to_stored(const void* blob, void* stored) const override { blob_to_stored_impl<R>(cfg, blob, stored, 0); }
   int chunks() const override { return R::kChunks; }
   void reset(const Ctx& c, long long n, cudaStream_t st) override {
     long long m = n > 0 ? n : 1;
@@ -698,6 +753,10 @@ struct GameOpsT : GameOps {
   void gather(const Ctx& dst, const Ctx& src, const long long* src_lanes, long long count, cudaStream_t st) override {
     if (count <= 0) return;
     k_gather<R><<<grid_for(count), kBlock, 0, st>>>(dst, src, src_lanes, count, cfg); ++g_launches;
+  }
+  void copy_to_blob(const Ctx& dst, const Ctx& src, long long count, cudaStream_t st) override {
+    if (count <= 0) return;
+    k_copy_to_blob<R><<<grid_for(count), kBlock, 0, st>>>(dst, src, count, cfg); ++g_launches;
   }
   void copy(const Ctx& dst, long long dst0, const Ctx& src, long long src0, long long count, cudaStream_t st) override {
     if (count <= 0) return;

@@ -106,6 +106,46 @@ __device__ __forceinline__ int rule_num_players_impl(const Cfg&, long) { return 
 template <class R, class Cfg>
 __device__ __forceinline__ int rule_num_players(const Cfg& c) { return rule_num_players_impl<R>(c, 0); }
 
+// Lane i's state in a batch <-> S.  A rule core stores a lane as it exchanges it (R::load / R::store on R::kChunks planes
+// of R::Chunk: the blob of b2s_state_get / b2s_state_set and of host States), unless it defines R::Packed: then a batch
+// holds one R::Packed per lane in a single plane, R::pack(s, cfg) encodes it and R::unpack(s, p, cfg) decodes it
+// (connect_four: the column height is in the configuration).  The streaming kernels fetch all their lanes before they
+// unpack any, so every load of a thread is in flight at once; Fetched<R> is what they hold in between.
+template <class R> auto fetched_of(int) -> typename R::Packed;
+template <class R> auto fetched_of(long) -> typename R::S;
+template <class R> using Fetched = decltype(fetched_of<R>(0));
+template <class R> auto stored_of(int) -> typename R::Packed;
+template <class R> auto stored_of(long) -> typename R::Chunk;
+template <class R> using StoredChunk = decltype(stored_of<R>(0));   // one chunk of a lane as a batch holds it
+template <class R, class P, class Q = typename R::Packed>
+__device__ __forceinline__ void fetch_state_impl(P& p, const Ctx& ctx, long long i, int) { p = reinterpret_cast<const Q*>(ctx.planes)[i]; }
+template <class R, class P>
+__device__ __forceinline__ void fetch_state_impl(P& p, const Ctx& ctx, long long i, long) { R::load(p, ctx, i); }
+template <class R, class P>
+__device__ __forceinline__ void fetch_state(P& p, const Ctx& ctx, long long i) { fetch_state_impl<R>(p, ctx, i, 0); }
+template <class R, class S, class P, class Cfg, class Q = typename R::Packed>
+__device__ __forceinline__ void unpack_state_impl(S& s, const P& p, const Cfg& c, int) { R::unpack(s, p, c); }
+template <class R, class S, class P, class Cfg>
+__device__ __forceinline__ void unpack_state_impl(S& s, const P& p, const Cfg&, long) { s = p; }
+template <class R, class S, class P, class Cfg>
+__device__ __forceinline__ void unpack_state(S& s, const P& p, const Cfg& c) { unpack_state_impl<R>(s, p, c, 0); }
+template <class R, class S, class Cfg, class Q = typename R::Packed>
+__device__ __forceinline__ void load_state_impl(S& s, const Cfg& c, const Ctx& ctx, long long i, int) {
+  R::unpack(s, reinterpret_cast<const Q*>(ctx.planes)[i], c);
+}
+template <class R, class S, class Cfg>
+__device__ __forceinline__ void load_state_impl(S& s, const Cfg&, const Ctx& ctx, long long i, long) { R::load(s, ctx, i); }
+template <class R, class S, class Cfg>
+__device__ __forceinline__ void load_state(S& s, const Cfg& c, const Ctx& ctx, long long i) { load_state_impl<R>(s, c, ctx, i, 0); }
+template <class R, class S, class Cfg, class Q = typename R::Packed>
+__device__ __forceinline__ void store_state_impl(const S& s, const Cfg& c, const Ctx& ctx, long long i, int) {
+  reinterpret_cast<Q*>(ctx.planes)[i] = R::pack(s, c);
+}
+template <class R, class S, class Cfg>
+__device__ __forceinline__ void store_state_impl(const S& s, const Cfg&, const Ctx& ctx, long long i, long) { R::store(s, ctx, i); }
+template <class R, class S, class Cfg>
+__device__ __forceinline__ void store_state(const S& s, const Cfg& c, const Ctx& ctx, long long i) { store_state_impl<R>(s, c, ctx, i, 0); }
+
 // One playout step: choose a uniformly random legal action and apply it; returns the action.
 // Rule cores may expose a cheap candidate superset (R::num_candidates / R::candidate, e.g. go: empty non-ko points
 // + pass) together with R::play_candidate, which applies the candidate or reports it illegal: a uniformly drawn

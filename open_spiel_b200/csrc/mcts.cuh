@@ -193,6 +193,7 @@ struct TreeArena {
   }
 };
 
+// rootctx holds the roots in the lane-blob form (R::load: b2s_mcts_search hands over a converted copy of the batch)
 template <class R, class NS, int MAXPATH, int MINBLOCKS>
 __global__ void __launch_bounds__(128, MINBLOCKS) k_mcts(Ctx rootctx, Ctx workctx, typename R::Cfg cfg, MctsArgs P, long long n_trees) {
   typedef typename NS::Node Node;

@@ -1,5 +1,6 @@
 // Microbenchmark (development tool, not part of the library): connect_four ApplyAction kernel variants on
-// rotating 1M-state batches inside a CUDA graph, to pick ILP / block size / launch attributes.
+// rotating 1M-state batches inside a CUDA graph, to pick ILP / block size / launch attributes: the earlier 16-byte
+// two-board lanes ({x, o}) and the library's 8-byte lanes.
 // nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o apply_variants apply_variants.cu
 #include <cstdio>
 #include <cstdlib>
@@ -88,7 +89,76 @@ __global__ void __launch_bounds__(BLOCK) k_apply_gs(ulonglong2* st, const int* _
   }
 }
 
+// ---- 8-byte lanes: the library's connect_four layout (rules_connect_four.cuh) at the default 6x7 ------------------------
+// key = x | (occ + BOTTOM): below a marker bit at its height, every column holds who owns each stone (1 = x); the cached
+// outcome sits in bits 62-63 as outcome ^ 2 (0 = game running).
+constexpr u64 BOTTOM = 0x40810204081ull;                                  // bit col*7
+constexpr u64 L1 = BOTTOM * 0x3f, L2 = BOTTOM * 0x1f, L4 = BOTTOM * 0x7;   // in-column rows < 6, < 5, < 3
+__device__ __forceinline__ bool step8(u64& key, int a, unsigned long long* err) {
+  if (a == -1) return false;
+  u64 s = key;
+  s |= (s >> 1) & L1; s |= (s >> 2) & L2; s |= (s >> 4) & L4;          // every column filled up to its marker
+  const u64 occ = (s >> 1) & L1;
+  u64 x = key & occ, o = occ & ~key;
+  if ((key >> 62) || a < 0 || a >= 7 || ((occ >> (a * 7 + 5)) & 1)) { atomicAdd(err, 1ull); return false; }
+  const u64 bit = (occ & (0x3full << (a * 7))) + (1ull << (a * 7));
+  const int mover = __popcll(occ) & 1;
+  const u64 mine = (mover ? o : x) | bit;
+  if (mover == 0) x = mine; else o = mine;
+  const int oc = has_line(mine) ? mover : (((occ | bit) & (BOTTOM << 5)) == (BOTTOM << 5) ? 3 : 2);
+  key = x | ((x | o) + BOTTOM) | ((u64)(oc ^ 2) << 62);
+  return true;
+}
+
+// one lane per 8-byte load, ILP lanes per thread (block-strided), MINB = __launch_bounds__ min blocks per SM
+template <int ILP, int BLOCK, int MINB>
+__global__ void __launch_bounds__(BLOCK, MINB) k_apply8(u64* st, const int* __restrict__ act, long long n, unsigned long long* err) {
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  long long base = (long long)blockIdx.x * (BLOCK * ILP) + threadIdx.x;
+  int a[ILP]; u64 s[ILP];
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) { long long i = base + (long long)j * BLOCK; a[j] = -1; if (i < n) { a[j] = __ldg(act + i); s[j] = st[i]; } }
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) { long long i = base + (long long)j * BLOCK; if (step8(s[j], a[j], err)) st[i] = s[j]; }
+}
+
+// two adjacent lanes per thread: one 16-byte state load / store and one 8-byte action load (n even)
+template <int ILP, int BLOCK, int MINB>
+__global__ void __launch_bounds__(BLOCK, MINB) k_apply8_pair(u64* st, const int* __restrict__ act, long long n, unsigned long long* err) {
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  long long base = (long long)blockIdx.x * (BLOCK * ILP) + threadIdx.x;
+  int2 a[ILP]; ulonglong2 s[ILP];
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) {
+    long long p = base + (long long)j * BLOCK;
+    a[j] = make_int2(-1, -1);
+    if (p < n / 2) { a[j] = __ldg(reinterpret_cast<const int2*>(act) + p); s[j] = reinterpret_cast<const ulonglong2*>(st)[p]; }
+  }
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) {
+    long long p = base + (long long)j * BLOCK;
+    bool w0 = step8(s[j].x, a[j].x, err), w1 = step8(s[j].y, a[j].y, err);
+    if (w0 || w1) reinterpret_cast<ulonglong2*>(st)[p] = s[j];
+  }
+}
+
+template <int ILP, int BLOCK, int MINB, bool PAIR>
+void launch8(void* st, const int* act, long long n, unsigned long long* err, cudaStream_t s) {
+  long long units = PAIR ? n / 2 : n;
+  unsigned grid = (unsigned)((units + (long long)BLOCK * ILP - 1) / ((long long)BLOCK * ILP));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(BLOCK); cfg.stream = s;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  if (PAIR) CK(cudaLaunchKernelEx(&cfg, k_apply8_pair<ILP, BLOCK, MINB>, (u64*)st, act, n, err));
+  else CK(cudaLaunchKernelEx(&cfg, k_apply8<ILP, BLOCK, MINB>, (u64*)st, act, n, err));
+}
+
 struct Variant { const char* name; void (*launch)(ulonglong2*, const int*, long long, unsigned long long*, cudaStream_t); };
+struct Variant8 { const char* name; void (*launch)(void*, const int*, long long, unsigned long long*, cudaStream_t); };
 
 template <int ILP, int BLOCK, bool PDL>
 void launch_v(ulonglong2* st, const int* act, long long n, unsigned long long* err, cudaStream_t s) {
@@ -158,6 +228,39 @@ int main(int argc, char** argv) {
     double us = best * 1e3 / K;
     printf("%-20s n=%lld  %.2f us/step  %.1f GB/s (36 B/step)  %.3e steps/s\n", v.name, n, us, 36.0 * n / us / 1e3, n / us * 1e6);
     CK(cudaGraphExecDestroy(ge)); CK(cudaGraphDestroy(g));
+  }
+  // ---- 8-byte lanes, the K steps captured as one chain and as two parallel chains (step k on chain k mod 2, as bench.py) --
+  Variant8 v8[] = {
+    {"c8_ilp4_b256_m6", launch8<4, 256, 6, false>}, {"c8_ilp8_b256_m1", launch8<8, 256, 1, false>},
+    {"c8_ilp8_b256_m4", launch8<8, 256, 4, false>}, {"c8_ilp8_b256_m6", launch8<8, 256, 6, false>},
+    {"c8_ilp16_b256_m1", launch8<16, 256, 1, false>}, {"c8_ilp8_b128_m1", launch8<8, 128, 1, false>},
+    {"c8_ilp4_b512_m1", launch8<4, 512, 1, false>},
+    {"c8_pair2_b256_m6", launch8<2, 256, 6, true>}, {"c8_pair4_b256_m1", launch8<4, 256, 1, true>},
+    {"c8_pair4_b256_m6", launch8<4, 256, 6, true>},
+  };
+  cudaStream_t s2; CK(cudaStreamCreate(&s2));
+  cudaEvent_t fork, join; CK(cudaEventCreateWithFlags(&fork, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&join, cudaEventDisableTiming));
+  for (int chains = 1; chains <= 2; ++chains) {
+    for (auto& v : v8) {
+      for (int k = 0; k < slots; ++k) CK(cudaMemsetAsync(st[k], 0, n * 8, s));    // all-zero keys decode to the empty board
+      cudaGraph_t g; cudaGraphExec_t ge;
+      CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeGlobal));
+      if (chains == 2) { CK(cudaEventRecord(fork, s)); CK(cudaStreamWaitEvent(s2, fork, 0)); }
+      for (int k = 10; k < slots; ++k) v.launch(st[k], act[k], n, err, (chains == 2 && (k & 1)) ? s2 : s);
+      if (chains == 2) { CK(cudaEventRecord(join, s2)); CK(cudaStreamWaitEvent(s, join, 0)); }
+      CK(cudaStreamEndCapture(s, &g)); CK(cudaGraphInstantiate(&ge, g, 0));
+      for (int k = 0; k < 10; ++k) v.launch(st[k], act[k], n, err, s);
+      float best = 1e9;
+      for (int rep = 0; rep < 3; ++rep) {
+        CK(cudaStreamSynchronize(s));
+        CK(cudaEventRecord(e0, s)); CK(cudaGraphLaunch(ge, s)); CK(cudaEventRecord(e1, s));
+        CK(cudaStreamSynchronize(s));
+        float ms; CK(cudaEventElapsedTime(&ms, e0, e1)); if (ms < best) best = ms;
+      }
+      double us = best * 1e3 / K;
+      printf("%-20s chains=%d n=%lld  %.2f us/step  %.1f GB/s (20 B/step)  %.3e steps/s\n", v.name, chains, n, us, 20.0 * n / us / 1e3, n / us * 1e6);
+      CK(cudaGraphExecDestroy(ge)); CK(cudaGraphDestroy(g));
+    }
   }
   // ---- dependent steps on ONE large batch (argv[3] lanes, default 16M): grid-wide PDL wait vs per-tile flags ----
   {
