@@ -138,7 +138,7 @@ def test_outcome_sampling_converges():
     assert t.nash_conv() < 2.0
 
 
-_DENSE_SCRIPT = r"""
+_HASH_SCRIPT = r"""
 import sys, hashlib
 import numpy as np
 sys.path.insert(0, sys.argv[1])
@@ -158,20 +158,19 @@ print(" ".join(out))
 """
 
 
-def test_delta_log_path_equals_dense_rows_bitwise():
-    """The three table-update paths add the same numbers in the same order — delta logs scattered into dense rows (default),
-    delta logs added lane by lane in shared memory (B2S_MCCFR_MODE=lanes), dense rows written by the traversals themselves
-    (B2S_MCCFR_MODE=dense, round 1): regret and average-policy tables hash-identical for external sampling (simple and full
-    averaging) and outcome sampling."""
+def test_lanes_path_equals_scatter_path_bitwise():
+    """The two table-update paths add the same numbers in the same order — delta logs scattered into dense rows (default),
+    delta logs added lane by lane in shared memory (B2S_MCCFR_MODE=lanes, chosen by default only for rows beyond 8 GiB):
+    regret and average-policy tables hash-identical for external sampling (simple and full averaging) and outcome sampling.
+    The scatter path itself is pinned to the oracle by the tests above."""
     import os
     import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     runs = []
-    for mode in ("scatter", "lanes", "dense"):
+    for mode in ("scatter", "lanes"):
         env = dict(os.environ, B2S_MCCFR_MODE=mode)
-        env.pop("B2S_MCCFR_DENSE", None)
-        r = subprocess.run([sys.executable, "-c", _DENSE_SCRIPT, root], capture_output=True, text=True, env=env, timeout=600)
+        r = subprocess.run([sys.executable, "-c", _HASH_SCRIPT, root], capture_output=True, text=True, env=env, timeout=600)
         assert r.returncode == 0, r.stderr[-2000:]
         runs.append(r.stdout.strip().split())
-    assert len(runs[0]) == 12 and runs[0] == runs[1] == runs[2]
+    assert len(runs[0]) == 12 and runs[0] == runs[1]
