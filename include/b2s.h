@@ -222,8 +222,9 @@ int b2s_record_trajectories(void* batch, uint64_t seed, int64_t lane_offset, int
  * Deterministic perfect-information games only (tic_tac_toe, connect_four, breakthrough, hex, go).
  * Every tree owns an arena of 16-byte nodes (24 bytes when n_rollouts is not a power of two); max_nodes_per_tree is the
  * reference's node budget with its garbage collection, max_nodes_total the physical arena size (0 = derived).  A tree
- * that cannot allocate stops and is counted by b2s_error_count.  Chance nodes in the tree, Dirichlet noise and custom
- * evaluators are not device features (the host adapters route such bots to the stock MCTSBot). */
+ * that cannot allocate stops and is counted by b2s_error_count.  Chance nodes in the tree are not a device feature; custom
+ * evaluators and Dirichlet noise are the b2s_mcts_eval_* search below (the host adapters route MCTSBots with per-state
+ * evaluators or Dirichlet noise to the stock MCTSBot). */
 enum { B2S_MCTS_UCT = 0, B2S_MCTS_PUCT = 1 };   /* UCTValue mcts.cc:90-101 / PUCTValue :103-112 (uniform prior, :74-87) */
 typedef struct b2s_mcts_config {
   int32_t max_simulations;
@@ -251,6 +252,53 @@ int b2s_mcts_search(void* roots_batch, int64_t n_trees, const b2s_mcts_config* c
                     void* stream);
 /* Arena nodes consumed by the last b2s_mcts_search on this batch (sum over trees of the arena high-water marks). */
 int b2s_mcts_nodes_used(void* roots_batch, int64_t* nodes);
+
+/* MCTSBot::MCTSearch (mcts.cc:353-467) with a CALLER-SUPPLIED Evaluator (mcts.h:83-92: Evaluate and Prior), e.g. a torch
+ * network, for n independent roots: the search runs on the device in rounds and hands its leaves to the caller in batches.
+ * Same games as b2s_mcts_search (poker games are rejected); no wall-clock budget (the caller owns the loop and the time).
+ *   b2s_mcts_eval_create  copies lanes [0, n_trees) of roots_batch into the search.  leaves_batch: a batch of the same game,
+ *                         parameters and device with capacity >= n_trees; the search writes the states it needs evaluated into
+ *                         its lanes (for go with the root's superko history plus the path's moves), so b2s_observation /
+ *                         b2s_legal_mask on it see the real states.  The caller must not write to it while the search lives.
+ *   b2s_mcts_eval_step    advances every live tree until it needs an evaluation or finishes (simulations that end at terminal
+ *                         states need none, so one step may run several).  pending_d [n] (nullable, device) = 1 where lane i of
+ *                         the leaves batch waits for an answer; n_pending_h (nullable, host; synchronises) = their number, 0 when
+ *                         the search is over.  values_d [n][num_players] and priors_d [n][num_distinct_actions] (float64, device,
+ *                         priors by action id) answer the previous step's pending lanes; NULL on the first step only; entries of
+ *                         other lanes and of illegal actions are ignored.  A request made at a leaf's first visit uses the value
+ *                         (Evaluate) and keeps the prior for the leaf's expansion at its second visit, so a caller evaluates each
+ *                         new node once; a node whose children or cached prior the garbage collector freed asks again at its
+ *                         next expansion and only the prior is used (prior-only request).
+ *   b2s_mcts_eval_results the root statistics with the layout and meaning of b2s_mcts_search's outputs (nullable: outcome_p0_d,
+ *                         best_action_d, sims_run_d, gc_runs_d); prior_requests_d [n] (nullable) = prior-only requests per
+ *                         tree.  Valid between steps (then the statistics so far).  Enqueued on `stream`.
+ * With a deterministic evaluator the trees equal the reference's MCTSBot with that Evaluator, on the position-keyed Philox
+ * stream of b2s_mcts_search for the child shuffles.  Nodes are 32 bytes (double total_reward and prior); a tree that cannot
+ * allocate stops and is counted by b2s_error_count on the leaves batch.  Dirichlet noise (mcts.cc:284-292): root_noise_d
+ * [n][num_distinct_actions] (float64, device, nullable; copied at create) is mixed into the root's priors at its expansion as
+ * (1 - dirichlet_epsilon) * prior + dirichlet_epsilon * noise[action]; the caller draws it (Dirichlet(alpha) over the legal
+ * actions).  Every step is one kernel launch; results one more. */
+typedef struct b2s_mcts_eval_config {
+  int32_t max_simulations;
+  int32_t solve;
+  int32_t child_selection_policy;   /* B2S_MCTS_UCT (the prior is unused, as in the reference) or B2S_MCTS_PUCT */
+  int32_t reserved0;                /* must be 0 */
+  double uct_c;
+  uint64_t seed;
+  int64_t tree_index_offset;        /* as b2s_mcts_config */
+  int64_t max_nodes_total;          /* as b2s_mcts_config (32-byte nodes; 0 = derived) */
+  int64_t max_nodes_per_tree;       /* MCTSBot::max_nodes_, as b2s_mcts_config */
+  double dirichlet_epsilon;
+  const double* root_noise_d;       /* nullable [n][num_distinct_actions] */
+} b2s_mcts_eval_config;
+int  b2s_mcts_eval_create(void* roots_batch, int64_t n_trees, const b2s_mcts_eval_config* cfg, void* leaves_batch,
+                          void** out_search, void* stream);
+int  b2s_mcts_eval_step(void* search, const double* values_d, const double* priors_d, uint8_t* pending_d,
+                        int64_t* n_pending_h, void* stream);
+int  b2s_mcts_eval_results(void* search, int32_t* visit_counts_d, double* total_reward_d, float* outcome_p0_d,
+                           int32_t* best_action_d, int32_t* sims_run_d, int32_t* gc_runs_d, int32_t* prior_requests_d,
+                           void* stream);
+void b2s_mcts_eval_destroy(void* search);
 
 /* ---- CFR ----------------------------------------------------------------------------------- */
 

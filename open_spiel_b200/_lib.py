@@ -44,6 +44,13 @@ class MctsConfig(C.Structure):
                 ("max_wall_clock_time", C.c_double), ("gc_runs_d", C.c_void_p)]
 
 
+class MctsEvalConfig(C.Structure):
+    _fields_ = [("max_simulations", C.c_int32), ("solve", C.c_int32), ("child_selection_policy", C.c_int32),
+                ("reserved0", C.c_int32), ("uct_c", C.c_double), ("seed", C.c_uint64), ("tree_index_offset", C.c_int64),
+                ("max_nodes_total", C.c_int64), ("max_nodes_per_tree", C.c_int64), ("dirichlet_epsilon", C.c_double),
+                ("root_noise_d", C.c_void_p)]
+
+
 class TrajectoryOut(C.Structure):
     _fields_ = [("observations", C.c_void_p), ("legal_mask", C.c_void_p), ("actions", C.c_void_p),
                 ("player_ids", C.c_void_p), ("valid", C.c_void_p), ("next_is_terminal", C.c_void_p),
@@ -88,6 +95,10 @@ SIGNATURES = {
     "b2s_mcts_search": (C.c_int, [_VP, _I64, C.POINTER(MctsConfig), _VP, _VP, _VP, _VP, _VP, _VP]),
     "b2s_mcts_nodes_used": (C.c_int, [_VP, C.POINTER(_I64)]),
     "b2s_gather_states": (C.c_int, [_VP, _VP, _VP, _I64, _VP]),
+    "b2s_mcts_eval_create": (C.c_int, [_VP, _I64, C.POINTER(MctsEvalConfig), _VP, C.POINTER(_VP), _VP]),
+    "b2s_mcts_eval_step": (C.c_int, [_VP, _VP, _VP, _VP, C.POINTER(_I64), _VP]),
+    "b2s_mcts_eval_results": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "b2s_mcts_eval_destroy": (None, [_VP]),
     "b2s_cfr_create": (C.c_int, [C.c_int, C.POINTER(Params), C.c_int, C.c_int, C.POINTER(_VP)]),
     "b2s_cfr_destroy": (None, [_VP]),
     "b2s_cfr_iterate": (C.c_int, [_VP, C.c_int, _VP]),

@@ -7,6 +7,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -700,6 +701,158 @@ int b2s_mcts_search(void* roots_batch, int64_t n_trees, const b2s_mcts_config* c
   CU(cudaStreamSynchronize(st));          // the search is a long-running call; results are ready on return
   return 0;
 }
+
+}  // extern "C"
+
+// ---- caller-evaluated MCTS (mcts_eval.cuh) ----------------------------------------------------------------------
+namespace b2s {
+struct MctsEvalSearch {
+  Batch* leaves = nullptr;
+  long long n = 0;
+  int max_legal = 0, max_path = 0, steps = 0;
+  MctsEvalArgs a;
+  void* roots = nullptr;            // the roots in the lane-blob form, leaves->cap lanes (lanes [0, n) used)
+  double* log_table = nullptr;
+  MctsNodeE* pool = nullptr;
+  MctsEvalTree* trees = nullptr;
+  u32* free_heads = nullptr;
+  u32* path = nullptr;
+  unsigned char* pending = nullptr;
+  unsigned long long* n_pending = nullptr;
+  double* noise = nullptr;
+  ~MctsEvalSearch() {
+    if (leaves) cudaSetDevice(leaves->device);
+    for (void* p : {(void*)roots, (void*)log_table, (void*)pool, (void*)trees, (void*)free_heads, (void*)path, (void*)pending,
+                    (void*)n_pending, (void*)noise})
+      if (p) cudaFree(p);
+  }
+  Ctx roots_ctx() const { Ctx c; c.planes = roots; c.cap = leaves->cap; c.hist = leaves->hist; c.err = leaves->err; return c; }
+};
+}  // namespace b2s
+
+extern "C" {
+
+int b2s_mcts_eval_create(void* roots_batch, int64_t n_trees, const b2s_mcts_eval_config* cfg, void* leaves_batch, void** out_search,
+                         void* stream) {
+  if (!out_search) return fail("mcts_eval: null out_search");
+  *out_search = nullptr;
+  if (int r = check(roots_batch, n_trees)) return r;
+  if (!cfg || !leaves_batch) return fail("mcts_eval: null argument");
+  Batch* B = (Batch*)roots_batch;
+  Batch* L = (Batch*)leaves_batch;
+  if (L->device != B->device || memcmp(&L->info, &B->info, sizeof(b2s_game_info)) != 0)
+    return fail("mcts_eval: the leaves batch must be of the same game, parameters and device as the roots batch");
+  if (n_trees < 1) return fail("mcts_eval: n_trees must be >= 1");
+  if (L->cap < n_trees) return fail("mcts_eval: the leaves batch holds fewer lanes than n_trees");
+  if (cfg->max_simulations < 1) return fail("mcts_eval: max_simulations must be >= 1");
+  if (cfg->max_nodes_per_tree < 0 || cfg->max_nodes_total < 0) return fail("mcts_eval: negative budget");
+  if (cfg->max_nodes_per_tree > 0x7fffffffll) return fail("mcts_eval: max_nodes_per_tree out of range");
+  if (cfg->child_selection_policy != B2S_MCTS_UCT && cfg->child_selection_policy != B2S_MCTS_PUCT)
+    return fail("mcts_eval: unknown child_selection_policy");
+  if (!(cfg->dirichlet_epsilon >= 0.0 && cfg->dirichlet_epsilon <= 1.0)) return fail("mcts_eval: dirichlet_epsilon must be in [0, 1]");
+  if (cfg->reserved0 != 0) return fail("mcts_eval: reserved0 must be 0");
+  int max_legal = 0, max_path = 0;
+  if (const char* e = B->ops->mcts_eval_limits(&max_legal, &max_path)) return fail(e);
+  cudaStream_t st = (cudaStream_t)stream;
+  std::unique_ptr<MctsEvalSearch> S(new MctsEvalSearch);
+  S->leaves = L; S->n = n_trees; S->max_legal = max_legal; S->max_path = max_path;
+  const size_t N = (size_t)n_trees, A = (size_t)B->info.num_distinct_actions;
+  // arena: every simulation allocates at most one block for an expansion and one for a prior cache; caches stop at half of it
+  const size_t node_bytes = sizeof(MctsNodeE);
+  unsigned long long per_tree;
+  if (cfg->max_nodes_total > 0) {
+    per_tree = (unsigned long long)cfg->max_nodes_total / (unsigned long long)n_trees;
+  } else {
+    const unsigned long long worst = 2ull + 2ull * (unsigned long long)cfg->max_simulations * A;
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    const unsigned long long fit = (unsigned long long)(free_b * 0.6 / node_bytes) / (unsigned long long)n_trees;
+    per_tree = worst < fit ? worst : fit;
+    if (cfg->max_nodes_per_tree > 1) {   // as b2s_mcts_search's budgeted arena (twice the budget), twice over for the caches
+      const unsigned long long want = 4ull * (unsigned long long)cfg->max_nodes_per_tree + 16 * A + 128;
+      if (want < per_tree) per_tree = want;
+    }
+  }
+  if (per_tree > 0xffffffffull) per_tree = 0xffffffffull;
+  if (per_tree < 2 * A + 2) return fail("mcts_eval: node arena too small (max_nodes_total / free memory)");
+  CU(cudaMalloc(&S->roots, (size_t)B->info.state_bytes * (size_t)L->cap));
+  CU(cudaMalloc((void**)&S->pool, per_tree * N * node_bytes));
+  CU(cudaMalloc((void**)&S->trees, sizeof(MctsEvalTree) * N));
+  CU(cudaMalloc((void**)&S->free_heads, sizeof(u32) * (size_t)(max_legal + 1) * N));
+  CU(cudaMalloc((void**)&S->path, sizeof(u32) * (size_t)max_path * N));
+  CU(cudaMalloc((void**)&S->pending, N));
+  CU(cudaMalloc((void**)&S->n_pending, sizeof(unsigned long long)));
+  {
+    const int need = cfg->max_simulations + 2;
+    std::vector<double> t(need);
+    for (int k = 0; k < need; ++k) t[k] = std::log((double)k);
+    CU(cudaMalloc((void**)&S->log_table, sizeof(double) * need));
+    CU(cudaMemcpyAsync(S->log_table, t.data(), sizeof(double) * need, cudaMemcpyHostToDevice, st));
+  }
+  if (cfg->root_noise_d) {         // the search keeps its own copy: the caller may reuse the buffer
+    CU(cudaMalloc((void**)&S->noise, sizeof(double) * A * N));
+    CU(cudaMemcpyAsync(S->noise, cfg->root_noise_d, sizeof(double) * A * N, cudaMemcpyDeviceToDevice, st));
+  }
+  CU(cudaMemsetAsync(S->trees, 0, sizeof(MctsEvalTree) * N, st));
+  CU(cudaMemsetAsync(S->pending, 0, N, st));
+  // roots -> blob lanes of the search; their superko histories (go) -> the leaves batch, where the descents extend them
+  B->ops->copy_to_blob(S->roots_ctx(), B->ctx(), n_trees, st);
+  if (int r = post()) return r;
+  MctsEvalArgs& a = S->a;
+  memset(&a, 0, sizeof a);
+  a.sims = cfg->max_simulations; a.solve = cfg->solve; a.num_actions = (int)A; a.mask_words = B->info.mask_words;
+  a.puct = cfg->child_selection_policy == B2S_MCTS_PUCT; a.max_nodes = (int)cfg->max_nodes_per_tree;
+  a.uct_c = cfg->uct_c; a.max_utility = B->info.max_utility; a.epsilon = cfg->dirichlet_epsilon;
+  a.seed = cfg->seed; a.tree_offset = cfg->tree_index_offset; a.log_table = S->log_table;
+  a.pool = S->pool; a.nodes_per_tree = per_tree; a.cache_cap = (u32)(per_tree / 2);
+  a.trees = S->trees; a.free_heads = S->free_heads; a.path = S->path; a.noise = S->noise;
+  a.pending = S->pending; a.n_pending = S->n_pending; a.err = L->err;
+  CU(cudaStreamSynchronize(st));
+  *out_search = S.release();
+  return 0;
+}
+
+int b2s_mcts_eval_step(void* search, const double* values_d, const double* priors_d, uint8_t* pending_d, int64_t* n_pending_h,
+                       void* stream) {
+  if (!search) return fail("mcts_eval: null search");
+  MctsEvalSearch* S = (MctsEvalSearch*)search;
+  if (S->steps > 0 && (!values_d || !priors_d)) return fail("mcts_eval: values and priors are required after the first step");
+  CU(cudaSetDevice(S->leaves->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  MctsEvalArgs a = S->a;
+  a.values = values_d; a.priors = priors_d;
+  CU(cudaMemsetAsync(S->n_pending, 0, sizeof(unsigned long long), st));
+  S->leaves->ops->mcts_eval_step(S->roots_ctx(), S->leaves->ctx(), S->n, a, st);
+  if (int r = post()) return r;
+  ++S->steps;
+  if (pending_d) CU(cudaMemcpyAsync(pending_d, S->pending, (size_t)S->n, cudaMemcpyDeviceToDevice, st));
+  if (n_pending_h) {
+    unsigned long long v = 0;
+    CU(cudaMemcpyAsync(&v, S->n_pending, sizeof v, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    *n_pending_h = (int64_t)v;
+  }
+  return 0;
+}
+
+int b2s_mcts_eval_results(void* search, int32_t* visit_counts_d, double* total_reward_d, float* outcome_p0_d, int32_t* best_action_d,
+                          int32_t* sims_run_d, int32_t* gc_runs_d, int32_t* prior_requests_d, void* stream) {
+  if (!search) return fail("mcts_eval: null search");
+  if (!visit_counts_d || !total_reward_d) return fail("mcts_eval: null argument");
+  MctsEvalSearch* S = (MctsEvalSearch*)search;
+  CU(cudaSetDevice(S->leaves->device));
+  MctsEvalArgs a = S->a;
+  a.visits_out = visit_counts_d; a.reward_out = total_reward_d; a.outcome_out = outcome_p0_d; a.best_out = best_action_d;
+  a.sims_out = sims_run_d; a.gc_out = gc_runs_d; a.prior_requests_out = prior_requests_d;
+  S->leaves->ops->mcts_eval_report(S->n, a, (cudaStream_t)stream);
+  return post();
+}
+
+void b2s_mcts_eval_destroy(void* search) { delete (MctsEvalSearch*)search; }
+
+}  // extern "C"
+
+extern "C" {
 
 int b2s_mcts_nodes_used(void* roots_batch, int64_t* nodes) {
   if (int r = check(roots_batch, 0)) return r;

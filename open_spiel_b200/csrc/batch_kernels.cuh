@@ -625,6 +625,11 @@ struct GameOps {
   virtual void traj_finish(const Ctx&, float* rewards, long long n, cudaStream_t) = 0;
   // MCTS over n roots (mcts.cuh); returns an error string when the game has no device MCTS
   virtual const char* mcts(const Ctx& roots, const Ctx& work, long long n, const struct MctsArgs& args, cudaStream_t) = 0;
+  // caller-evaluated MCTS (mcts_eval.cuh): the children-block and path-stack sizes of the game's device search, or an error
+  // string when it has none; one resumable step of n trees; the root statistics
+  virtual const char* mcts_eval_limits(int* max_legal, int* max_path) const = 0;
+  virtual void mcts_eval_step(const Ctx& roots, const Ctx& leaves, long long n, const struct MctsEvalArgs& args, cudaStream_t) = 0;
+  virtual void mcts_eval_report(long long n, const struct MctsEvalArgs& args, cudaStream_t) = 0;
   b2s_game_info info;
 };
 
@@ -750,6 +755,9 @@ struct GameOpsT : GameOps {
     k_traj_finish<R><<<grid_for(n), kBlock, 0, st>>>(c, cfg, rewards, n); ++g_launches;
   }
   const char* mcts(const Ctx& roots, const Ctx& work, long long n, const MctsArgs& args, cudaStream_t st) override;
+  const char* mcts_eval_limits(int* max_legal, int* max_path) const override;
+  void mcts_eval_step(const Ctx& roots, const Ctx& leaves, long long n, const MctsEvalArgs& args, cudaStream_t st) override;
+  void mcts_eval_report(long long n, const MctsEvalArgs& args, cudaStream_t st) override;
   void gather(const Ctx& dst, const Ctx& src, const long long* src_lanes, long long count, cudaStream_t st) override {
     if (count <= 0) return;
     k_gather<R><<<grid_for(count), kBlock, 0, st>>>(dst, src, src_lanes, count, cfg); ++g_launches;
@@ -766,6 +774,7 @@ struct GameOpsT : GameOps {
 
 }  // namespace b2s
 #include "mcts.cuh"
+#include "mcts_eval.cuh"
 namespace b2s {
 template <class R>
 const char* GameOpsT<R>::mcts(const Ctx& roots, const Ctx& work, long long n, const MctsArgs& args, cudaStream_t st) {
@@ -791,6 +800,33 @@ const char* GameOpsT<R>::mcts(const Ctx& roots, const Ctx& work, long long n, co
     return nullptr;
   } else {
     return "mcts: games with chance nodes / imperfect information have no device MCTS";
+  }
+}
+
+template <class R>
+const char* GameOpsT<R>::mcts_eval_limits(int* max_legal, int* max_path) const {
+  if constexpr (R::kMaxPath > 0) {
+    if (info.max_game_length + 2 > R::kMaxPath) return "mcts_eval: max_game_length too large for the device search path stack";
+    if (info.min_utility != -1.0 || info.max_utility != 1.0) return "mcts_eval: the device search needs win / loss / draw returns";
+    *max_legal = R::kMaxLegal;
+    *max_path = R::kMaxPath;
+    return nullptr;
+  } else {
+    return "mcts_eval: games with chance nodes / imperfect information have no device MCTS";
+  }
+}
+template <class R>
+void GameOpsT<R>::mcts_eval_step(const Ctx& roots, const Ctx& leaves, long long n, const MctsEvalArgs& args, cudaStream_t st) {
+  if constexpr (R::kMaxPath > 0) {
+    if (n <= 0) return;
+    k_mcts_eval_step<R, R::kMaxPath><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(roots, leaves, cfg, args, n); ++g_launches;
+  }
+}
+template <class R>
+void GameOpsT<R>::mcts_eval_report(long long n, const MctsEvalArgs& args, cudaStream_t st) {
+  if constexpr (R::kMaxPath > 0) {
+    if (n <= 0) return;
+    k_mcts_eval_report<R><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(args, n); ++g_launches;
   }
 }
 

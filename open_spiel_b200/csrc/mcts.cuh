@@ -28,8 +28,8 @@
 // Selection is the reference's first-maximum scan in FP64 (an unvisited child is +infinity, so the first unvisited child ends
 // the scan).  A float32 pre-selection with a proven error margin (FP64 only for children whose estimate could still win) was
 // tried and removed.
-// Not implemented: chance nodes in the tree, Dirichlet noise, custom evaluators (the host adapters route those to the
-// stock MCTSBot).
+// Not implemented here: chance nodes in the tree.  Custom evaluators and Dirichlet noise are the caller-evaluated search of
+// mcts_eval.cuh (b2s_mcts_eval_*); the host adapters still route MCTSBots with per-state evaluators to the stock MCTSBot.
 #pragma once
 #include "common.cuh"
 
@@ -164,11 +164,13 @@ __device__ __forceinline__ double exact_value(const typename NS::Node& ch, doubl
   return __dadd_rn(q, __dmul_rn(P.uct_c, u));
 }
 // Children block allocator of one tree (thread-private): exact-size free list, else bump, else split a larger free block.
-template <class Node, int KMAX>
+// Heads: the free-list heads, in registers / local memory (k_mcts) or a u32* into global memory (k_mcts_eval_step, whose
+// trees outlive a launch).
+template <class Node, int KMAX, class Heads = u32[KMAX + 1]>
 struct TreeArena {
   Node* pool;
   u32 cap, top;
-  u32 free_head[KMAX + 1];          // free_head[k]: first free block of exactly k nodes (chained through first_child), 0 = none
+  Heads free_head;                  // free_head[k]: first free block of exactly k nodes (chained through first_child), 0 = none
   __device__ __forceinline__ void init(Node* p, u32 capacity) {
     pool = p; cap = capacity; top = 1;
     for (int k = 0; k <= KMAX; ++k) free_head[k] = 0;

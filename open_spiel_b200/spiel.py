@@ -512,6 +512,122 @@ def mcts_search(batch, max_simulations, uct_c=2.0, n_rollouts=1, solve=True, see
     return out
 
 
+class MCTSEvalSearch:
+    """MCTSBot.MCTSearch (algorithms/mcts.cc:353-467) with a caller-supplied evaluator over n roots at once, driven in rounds
+    (b2s_mcts_eval_*): every step() advances all live trees until each needs an evaluation or finishes; the states to evaluate
+    are lanes of `.leaves` (a BatchedState of the roots' game), flagged by the returned `pending` mask.  The next step() takes
+    the answers: values [n, num_players] and priors [n, num_distinct_actions] (float64 device tensors, priors by action id;
+    rows of lanes that are not pending and entries of illegal actions are ignored).  step(None, None) starts the search.
+    With a deterministic evaluator the trees equal the reference MCTSBot's with that Evaluator (child shuffles on the
+    position-keyed stream of mcts_search).  root_noise [n, A] (float64, optional) is the root's Dirichlet noise, mixed in as
+    (1 - dirichlet_epsilon) * prior + dirichlet_epsilon * noise (see dirichlet_noise()).  max_wall_clock_time is not
+    supported: the caller owns the loop and its time budget."""
+
+    def __init__(self, roots_batch, max_simulations, uct_c=2.0, solve=True, seed=0, tree_index_offset=0, n_trees=None,
+                 child_selection_policy=ChildSelectionPolicy.UCT, max_nodes_per_tree=0, max_nodes_total=0, root_noise=None,
+                 dirichlet_epsilon=0.0, leaves=None, max_wall_clock_time=0.0):
+        from ._lib import MctsEvalConfig
+        if max_wall_clock_time:
+            raise B2SError("mcts_eval: max_wall_clock_time is not supported (the caller drives the rounds and owns the time budget)")
+        self._h = C.c_void_p()
+        self.n = roots_batch.n if n_trees is None else int(n_trees)
+        self.info = roots_batch.info
+        self._dev = roots_batch._dev
+        self.leaves = leaves if leaves is not None else BatchedState(roots_batch.game, self.n, roots_batch.device)
+        A = self.info.num_distinct_actions
+        noise_ptr = None
+        if root_noise is not None:
+            if root_noise.dtype != torch.float64 or not root_noise.is_cuda or tuple(root_noise.shape) != (self.n, A):
+                raise B2SError("mcts_eval: root_noise must be a float64 CUDA tensor of shape [n_trees, num_distinct_actions]")
+            root_noise = root_noise.contiguous()
+            noise_ptr = root_noise.data_ptr()
+        cfg = MctsEvalConfig(int(max_simulations), int(bool(solve)), int(child_selection_policy), 0, float(uct_c), int(seed),
+                             int(tree_index_offset), int(max_nodes_total), int(max_nodes_per_tree), float(dirichlet_epsilon),
+                             noise_ptr)
+        check(lib().b2s_mcts_eval_create(roots_batch._h, self.n, C.byref(cfg), self.leaves._h, C.byref(self._h),
+                                         self.leaves._stream()))
+        self._pending = torch.zeros((self.n,), dtype=torch.uint8, device=self._dev)
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib().b2s_mcts_eval_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def step(self, values=None, priors=None):
+        """One round.  Returns (pending [n] bool tensor, number of pending lanes); 0 pending = the search is over."""
+        ptrs = []
+        for name, t, width in (("values", values, self.info.num_players), ("priors", priors, self.info.num_distinct_actions)):
+            if t is None:
+                ptrs.append(None)
+                continue
+            if t.dtype != torch.float64 or not t.is_cuda or t.dim() != 2 or t.shape[0] < self.n or t.shape[1] != width:
+                raise B2SError("mcts_eval: %s must be a float64 CUDA tensor of shape [n_trees, %d]" % (name, width))
+            if not t.is_contiguous():
+                raise B2SError("mcts_eval: %s must be contiguous" % name)
+            ptrs.append(t.data_ptr())
+        n_pending = C.c_int64()
+        check(lib().b2s_mcts_eval_step(self._h, ptrs[0], ptrs[1], self._pending.data_ptr(), C.byref(n_pending), self.leaves._stream()))
+        return self._pending.bool(), n_pending.value
+
+    def results(self):
+        """The root statistics so far, as mcts_search returns them (visits, total_reward, outcome_p0, best_action, sims_run,
+        gc_runs), plus prior_requests [n] int32: prior-only requests (expansions after a garbage collection freed a node's
+        children or cached prior)."""
+        n, A, dev = self.n, self.info.num_distinct_actions, self._dev
+        out = {
+            "visits": torch.empty((n, A), dtype=torch.int32, device=dev),
+            "total_reward": torch.empty((n, A), dtype=torch.float64, device=dev),
+            "outcome_p0": torch.empty((n, A), dtype=torch.float32, device=dev),
+            "best_action": torch.empty((n,), dtype=torch.int32, device=dev),
+            "sims_run": torch.empty((n,), dtype=torch.int32, device=dev),
+            "gc_runs": torch.empty((n,), dtype=torch.int32, device=dev),
+            "prior_requests": torch.empty((n,), dtype=torch.int32, device=dev),
+        }
+        check(lib().b2s_mcts_eval_results(self._h, *[out[k].data_ptr() for k in ("visits", "total_reward", "outcome_p0", "best_action",
+                                                                                  "sims_run", "gc_runs", "prior_requests")],
+                                          self.leaves._stream()))
+        return out
+
+
+def mcts_search_evaluated(batch, evaluate, max_simulations, uct_c=2.0, solve=True, seed=0, tree_index_offset=0, n_trees=None,
+                          child_selection_policy=ChildSelectionPolicy.UCT, max_nodes_per_tree=0, max_nodes_total=0,
+                          root_noise=None, dirichlet_epsilon=0.0, leaves=None, max_wall_clock_time=0.0):
+    """Batched MCTSBot.mcts_search with a caller-supplied batched evaluator: `evaluate(leaves, pending) -> (values, priors)`
+    gets the leaves BatchedState and the pending mask (device tensors) and returns values [n, num_players] and priors
+    [n, num_distinct_actions] for the pending lanes (as MCTSEvalSearch.step takes them; other float dtypes are converted).
+    Runs the rounds until every tree has finished and returns MCTSEvalSearch.results() plus "rounds" (evaluate calls) and
+    "failed_trees" (trees that stopped because their node arena was full)."""
+    search = MCTSEvalSearch(batch, max_simulations, uct_c, solve, seed, tree_index_offset, n_trees, child_selection_policy,
+                            max_nodes_per_tree, max_nodes_total, root_noise, dirichlet_epsilon, leaves, max_wall_clock_time)
+    values = priors = None
+    rounds = 0
+    while True:
+        pending, n_pending = search.step(values, priors)
+        if n_pending == 0:
+            break
+        rounds += 1
+        values, priors = evaluate(search.leaves, pending)
+        values = values.to(torch.float64).contiguous()
+        priors = priors.to(torch.float64).contiguous()
+    out = search.results()
+    out["rounds"] = rounds
+    out["failed_trees"] = search.leaves.error_count()[0]    # trees that ran out of arena nodes (b2s_error_count)
+    return out
+
+
+def dirichlet_noise(batch, alpha, generator=None, n=None):
+    """Per lane a Dirichlet(alpha) vector over the lane's legal actions, scattered by action id ([n, A] float64, zero on illegal
+    actions): the noise dirichlet_noise (algorithms/mcts.cc:188-203) draws for the root, here drawn in torch as normalised
+    Gamma(alpha, 1) variates (torch's own stream, optionally `generator`)."""
+    mask = batch.legal_actions_mask(n=n).to(torch.float64)
+    conc = torch.full(mask.shape, float(alpha), dtype=torch.float64, device=mask.device)
+    g = torch._standard_gamma(conc, generator=generator) * mask
+    return g / g.sum(dim=1, keepdim=True).clamp_min(torch.finfo(torch.float64).tiny)
+
+
 def bind_host_to_device(device=0):
     """Pins the calling thread to the CPUs of the GPU's NUMA node (b2s_bind_host_to_device); returns the CPU count,
     or 0 when the topology cannot be read (containers without sysfs PCI entries)."""
