@@ -84,7 +84,7 @@ static GameOps* make_ops(int id, const b2s_params* p) {
     case B2S_CONNECT_FOUR: return make_ops_connect_four();
     case B2S_BREAKTHROUGH: return make_ops_breakthrough();
     case B2S_HEX: return make_ops_hex();
-    case B2S_GO: return make_ops_go();
+    case B2S_GO: return (!p || p->board_size < 0 || p->board_size > 9) ? make_ops_go_wide() : make_ops_go();
     case B2S_KUHN_POKER: return make_ops_kuhn_poker();
     case B2S_MNK: return make_ops_mnk();
     case B2S_OTHELLO: return make_ops_othello();

@@ -836,6 +836,7 @@ GameOps* make_ops_connect_four();
 GameOps* make_ops_breakthrough();
 GameOps* make_ops_hex();
 GameOps* make_ops_go();
+GameOps* make_ops_go_wide();    // board_size unset (19) or 10..19
 GameOps* make_ops_kuhn_poker();
 GameOps* make_ops_leduc_poker();
 GameOps* make_ops_leduc_poker_n();   // players = 3..4

@@ -205,6 +205,92 @@ __device__ __forceinline__ int b_select(B128 a, int k) {
   return 96 + (int)__fns((u32)(a.hi >> 32), 0, k + 1);
 }
 __device__ __forceinline__ int b_ffs(B128 a) { return a.lo ? __ffsll((long long)a.lo) - 1 : 64 + __ffsll((long long)a.hi) - 1; }
+__host__ __device__ __forceinline__ bool b_eq(B128 a, B128 b) { return a.lo == b.lo && a.hi == b.hi; }
+
+// ---- 384-bit bitboards (go 10..19: 19 rows x 20-bit stride) ------------------------------------------------------
+// Same names as B128's helpers.  Every word index is a compile-time constant (unrolled loops, no a.w[i >> 6] with a run-time
+// i), so a B384 stays in registers on the device.
+struct B384 {
+  u64 w[6];
+};
+__host__ __device__ __forceinline__ B384 b_and(const B384& a, const B384& b) {
+  B384 r;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) r.w[k] = a.w[k] & b.w[k];
+  return r;
+}
+__host__ __device__ __forceinline__ B384 b_or(const B384& a, const B384& b) {
+  B384 r;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) r.w[k] = a.w[k] | b.w[k];
+  return r;
+}
+__host__ __device__ __forceinline__ B384 b_andn(const B384& a, const B384& b) {   // a & ~b
+  B384 r;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) r.w[k] = a.w[k] & ~b.w[k];
+  return r;
+}
+__host__ __device__ __forceinline__ bool b_any(const B384& a) { return (a.w[0] | a.w[1] | a.w[2] | a.w[3] | a.w[4] | a.w[5]) != 0; }
+__host__ __device__ __forceinline__ bool b_eq(const B384& a, const B384& b) {
+  return ((a.w[0] ^ b.w[0]) | (a.w[1] ^ b.w[1]) | (a.w[2] ^ b.w[2]) | (a.w[3] ^ b.w[3]) | (a.w[4] ^ b.w[4]) | (a.w[5] ^ b.w[5])) == 0;
+}
+__host__ __device__ __forceinline__ B384 b_shl(const B384& a, int s) {   // 0 < s < 64
+  B384 r;
+  r.w[0] = a.w[0] << s;
+#pragma unroll
+  for (int k = 1; k < 6; ++k) r.w[k] = (a.w[k] << s) | (a.w[k - 1] >> (64 - s));
+  return r;
+}
+__host__ __device__ __forceinline__ B384 b_shr(const B384& a, int s) {   // 0 < s < 64
+  B384 r;
+#pragma unroll
+  for (int k = 0; k < 5; ++k) r.w[k] = (a.w[k] >> s) | (a.w[k + 1] << (64 - s));
+  r.w[5] = a.w[5] >> s;
+  return r;
+}
+// b_bit<B>(i): the one-bit set of either width (code generic over the set type); b_bit(i) stays the B128 one
+template <class B> __host__ __device__ __forceinline__ B b_bit(int i);
+template <> __host__ __device__ __forceinline__ B128 b_bit<B128>(int i) { return b_bit(i); }
+template <> __host__ __device__ __forceinline__ B384 b_bit<B384>(int i) {
+  B384 r;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) r.w[k] = (i >> 6) == k ? 1ull << (i & 63) : 0ull;
+  return r;
+}
+__host__ __device__ __forceinline__ bool b_test(const B384& a, int i) {
+  u64 v = 0;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) v |= (i >> 6) == k ? a.w[k] : 0ull;
+  return (v >> (i & 63)) & 1ull;
+}
+__device__ __forceinline__ int b_popc(const B384& a) {
+  return __popcll(a.w[0]) + __popcll(a.w[1]) + __popcll(a.w[2]) + __popcll(a.w[3]) + __popcll(a.w[4]) + __popcll(a.w[5]);
+}
+// position of the k-th (0-based) set bit; k < popcount
+__device__ __forceinline__ int b_select(const B384& a, int k) {
+  int base = 0;
+  u32 word = 0;
+  bool found = false;
+#pragma unroll
+  for (int h = 0; h < 12; ++h) {
+    const u32 x = (u32)(a.w[h >> 1] >> (32 * (h & 1)));
+    const int c = __popc(x);
+    if (!found) {
+      if (k < c) { found = true; word = x; base = 32 * h; }
+      else k -= c;
+    }
+  }
+  return base + (int)__fns(word, 0, k + 1);
+}
+// lowest set bit; the set must not be empty
+__device__ __forceinline__ int b_ffs(const B384& a) {
+  int r = 0;
+#pragma unroll
+  for (int k = 5; k >= 0; --k)
+    if (a.w[k]) r = 64 * k + __ffsll((long long)a.w[k]) - 1;
+  return r;
+}
 
 // ---- 256-bit bitboards (mnk: 15 rows x 16-bit stride; havannah: up to 15 x 15 cells) ---------------------------------
 struct B256 {

@@ -31,20 +31,29 @@
 // Not implemented here: chance nodes in the tree.  Custom evaluators and Dirichlet noise are the caller-evaluated search of
 // mcts_eval.cuh (b2s_mcts_eval_*); the host adapters still route MCTSBots with per-state evaluators to the stock MCTSBot.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace b2s {
 
-// meta word of a node: action (10 bits) | number of children (8) | player who chose the action (1) | proven (1) | outcome (2)
+// meta word of a node: action (10 bits) | number of children (9) | player who chose the action (1) | proven (1) | outcome (2);
+// bits 23-31 are free.  Nine child-count bits hold go 19x19's 362 children.
 // outcome: 0 = draw {0,0}, 1 = player 0 won {+1,-1}, 2 = player 1 won {-1,+1}
+constexpr int kMetaMaxChildren = 511;
 __host__ __device__ __forceinline__ u32 mcts_meta(int action, int nchild, int player, int proven, int outcome) {
-  return (u32)(action & 1023) | (u32)nchild << 10 | (u32)player << 18 | (u32)proven << 19 | (u32)outcome << 20;
+  return (u32)(action & 1023) | (u32)nchild << 10 | (u32)player << 19 | (u32)proven << 20 | (u32)outcome << 21;
 }
 __host__ __device__ __forceinline__ int meta_action(u32 m) { return (int)(m & 1023); }
-__host__ __device__ __forceinline__ int meta_nchild(u32 m) { return (int)((m >> 10) & 255); }
-__host__ __device__ __forceinline__ int meta_player(u32 m) { return (int)((m >> 18) & 1); }
-__host__ __device__ __forceinline__ int meta_proven(u32 m) { return (int)((m >> 19) & 1); }
-__host__ __device__ __forceinline__ int meta_outcome(u32 m) { return (int)((m >> 20) & 3); }
+__host__ __device__ __forceinline__ int meta_nchild(u32 m) { return (int)((m >> 10) & 511); }
+__host__ __device__ __forceinline__ int meta_player(u32 m) { return (int)((m >> 19) & 1); }
+__host__ __device__ __forceinline__ int meta_proven(u32 m) { return (int)((m >> 20) & 1); }
+__host__ __device__ __forceinline__ int meta_outcome(u32 m) { return (int)((m >> 21) & 3); }
+// the same word with `n` children / proven with outcome `code`
+__host__ __device__ __forceinline__ u32 meta_set_nchild(u32 m, int n) { return (m & ~(511u << 10)) | (u32)n << 10; }
+__host__ __device__ __forceinline__ u32 meta_set_proven(u32 m, int code) { return (m & ~(7u << 20)) | 1u << 20 | (u32)code << 21; }
+// child cursor of the collector's depth-first walk: one byte per stack level unless a node can have more than 255 children
+template <int KMAX> using GcCursor = typename std::conditional<(KMAX > 255), unsigned short, unsigned char>::type;
 // value of a proven outcome for player p: +1 / -1 / 0
 __host__ __device__ __forceinline__ int outcome_value(int code, int p) { return code == 0 ? 0 : ((code == 1) == (p == 0) ? 1 : -1); }
 
@@ -235,7 +244,7 @@ __global__ void __launch_bounds__(128, MINBLOCKS) k_mcts(Ctx rootctx, Ctx workct
   }
   const double inv_rollouts = __ddiv_rn(1.0, (double)P.n_rollouts);
   u32 path[MAXPATH];
-  unsigned char gc_iter[MAXPATH];                  // child cursor per stack level of the collector's depth-first walk
+  GcCursor<R::kMaxLegal> gc_iter[MAXPATH];         // child cursor per stack level of the collector's depth-first walk
   u32 expansions = 0;
   int nodes = 1;                                   // MCTSBot::nodes_
   int gc_limit = 5, gc_runs = 0;                   // MCTSBot::gc_limit_ (MIN_GC_LIMIT, mcts.cc:37)
@@ -270,7 +279,7 @@ __global__ void __launch_bounds__(128, MINBLOCKS) k_mcts(Ctx rootctx, Ctx workct
             ++n;
           }
         }
-        if (n > R::kMaxLegal || n > 255 || depth >= MAXPATH - 1) { failed = true; break; }
+        if (n > R::kMaxLegal || n > kMetaMaxChildren || depth >= MAXPATH - 1) { failed = true; break; }
         u32 base = arena.alloc(n);
         if (!base) { failed = true; break; }
         u32 e = expansions++;
@@ -287,7 +296,7 @@ __global__ void __launch_bounds__(128, MINBLOCKS) k_mcts(Ctx rootctx, Ctx workct
           pool[base + k] = c;
         }
         nd.first_child = base;
-        nd.meta = (nd.meta & ~(255u << 10)) | (u32)n << 10;
+        nd.meta = meta_set_nchild(nd.meta, n);
         pool[cur].first_child = nd.first_child;
         pool[cur].meta = nd.meta;
         nodes += n;                                 // nodes_ += children.capacity()
@@ -323,7 +332,7 @@ __global__ void __launch_bounds__(128, MINBLOCKS) k_mcts(Ctx rootctx, Ctx workct
       ret.val[0] = r[0]; ret.val[1] = r[1];
       ret.num[0] = (int)r[0] * P.n_rollouts; ret.num[1] = (int)r[1] * P.n_rollouts;
       const int code = r[0] > 0.f ? 1 : (r[0] < 0.f ? 2 : 0);
-      pool[cur].meta = (pool[cur].meta & ~(7u << 19)) | 1u << 19 | (u32)code << 20;
+      pool[cur].meta = meta_set_proven(pool[cur].meta, code);
       solved = P.solve != 0;
     } else {
       ret.val[0] = 0; ret.val[1] = 0; ret.num[0] = 0; ret.num[1] = 0;
@@ -367,7 +376,7 @@ __global__ void __launch_bounds__(128, MINBLOCKS) k_mcts(Ctx rootctx, Ctx workct
           }
         }
         if (best >= 0 && (all_solved || (double)best_v == P.max_utility)) {
-          nd.meta = (nd.meta & ~(7u << 19)) | 1u << 19 | (u32)best_code << 20;
+          nd.meta = meta_set_proven(nd.meta, best_code);
         } else {
           solved = false;
         }
@@ -395,7 +404,7 @@ __global__ void __launch_bounds__(128, MINBLOCKS) k_mcts(Ctx rootctx, Ctx workct
           arena.release(nd.first_child, nch);
           nodes -= nch;
           pool[ni].first_child = 0;
-          pool[ni].meta = nd.meta & ~(255u << 10);
+          pool[ni].meta = meta_set_nchild(nd.meta, 0);
         }
         --sp;
       }

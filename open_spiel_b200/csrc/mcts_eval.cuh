@@ -190,7 +190,7 @@ __global__ void __launch_bounds__(128) k_mcts_eval_step(Ctx roots, Ctx leaves, t
             break;
           }
           const int n = eval_legal_list<R>(s, cfg, P.mask_words, acts);
-          if (n > R::kMaxLegal || n > 255 || depth >= MAXPATH - 1) { failed = true; break; }
+          if (n > R::kMaxLegal || n > kMetaMaxChildren || depth >= MAXPATH - 1) { failed = true; break; }
           u32 base = nd.ncache ? nd.first_child : 0u;
           if (!base) {                             // Evaluator::Prior from this round's answer
             base = arena.alloc(n);
@@ -220,7 +220,7 @@ __global__ void __launch_bounds__(128) k_mcts_eval_step(Ctx roots, Ctx leaves, t
           }
           nd.first_child = base;
           nd.ncache = 0;
-          nd.meta = (nd.meta & ~(255u << 10)) | (u32)n << 10;
+          nd.meta = meta_set_nchild(nd.meta, n);
           pool[cur].first_child = base;
           pool[cur].ncache = 0;
           pool[cur].meta = nd.meta;
@@ -251,7 +251,7 @@ __global__ void __launch_bounds__(128) k_mcts_eval_step(Ctx roots, Ctx leaves, t
         R::returns(s, cfg, r);
         val[0] = r[0]; val[1] = r[1];
         const int code = r[0] > 0.f ? 1 : (r[0] < 0.f ? 2 : 0);
-        pool[cur].meta = (pool[cur].meta & ~(7u << 19)) | 1u << 19 | (u32)code << 20;
+        pool[cur].meta = meta_set_proven(pool[cur].meta, code);
         solved = P.solve != 0;
       } else {                                     // a leaf's first visit: ask for Evaluate (and Prior)
         store_state<R>(s, cfg, leaves, tree);
@@ -280,7 +280,7 @@ __global__ void __launch_bounds__(128) k_mcts_eval_step(Ctx roots, Ctx leaves, t
             if (best < 0 || v > best_v) { best = i; best_v = v; best_code = meta_outcome(cm); }
           }
         }
-        if (best >= 0 && (all_solved || (double)best_v == P.max_utility)) nd.meta = (nd.meta & ~(7u << 19)) | 1u << 19 | (u32)best_code << 20;
+        if (best >= 0 && (all_solved || (double)best_v == P.max_utility)) nd.meta = meta_set_proven(nd.meta, best_code);
         else solved = false;
       }
       pool[ni] = nd;
@@ -294,7 +294,7 @@ __global__ void __launch_bounds__(128) k_mcts_eval_step(Ctx roots, Ctx leaves, t
     // ---- node budget (mcts.cc:441-463): GarbageCollect (:469-482) plus every cached prior it reaches ----
     if (P.max_nodes > 1 && T.nodes >= P.max_nodes) {
       u32 stk[MAXPATH];
-      unsigned char it[MAXPATH];
+      GcCursor<R::kMaxLegal> it[MAXPATH];
       int sp = 0;
       stk[0] = 0; it[0] = 0;
       while (sp >= 0) {
@@ -317,7 +317,7 @@ __global__ void __launch_bounds__(128) k_mcts_eval_step(Ctx roots, Ctx leaves, t
           arena.release(nd.first_child, nch);
           T.nodes -= nch;
           pool[ni].first_child = 0;
-          pool[ni].meta = nd.meta & ~(255u << 10);
+          pool[ni].meta = meta_set_nchild(nd.meta, 0);
         }
         --sp;
       }
