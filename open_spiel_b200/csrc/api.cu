@@ -81,7 +81,9 @@ struct Batch {
 static GameOps* make_ops(int id, const b2s_params* p) {
   switch (id) {
     case B2S_TIC_TAC_TOE: return make_ops_tic_tac_toe();
-    case B2S_CONNECT_FOUR: return make_ops_connect_four();
+    case B2S_CONNECT_FOUR:   // the default board has its own instantiation with compile-time sizes (rules_connect_four.cuh)
+      return (!p || ((p->rows < 0 || p->rows == 6) && (p->columns < 0 || p->columns == 7) && (p->x_in_row < 0 || p->x_in_row == 4)))
+                 ? make_ops_connect_four_std() : make_ops_connect_four();
     case B2S_BREAKTHROUGH: return make_ops_breakthrough();
     case B2S_HEX: return make_ops_hex();
     case B2S_GO: return (!p || p->board_size < 0 || p->board_size > 9) ? make_ops_go_wide() : make_ops_go();

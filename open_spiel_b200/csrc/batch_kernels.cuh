@@ -833,6 +833,7 @@ void GameOpsT<R>::mcts_eval_report(long long n, const MctsEvalArgs& args, cudaSt
 // one factory per game, defined in game_<name>.cu
 GameOps* make_ops_tic_tac_toe();
 GameOps* make_ops_connect_four();
+GameOps* make_ops_connect_four_std();   // rows, columns, x_in_row unset or 6, 7, 4
 GameOps* make_ops_breakthrough();
 GameOps* make_ops_hex();
 GameOps* make_ops_go();

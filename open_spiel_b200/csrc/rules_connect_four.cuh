@@ -12,12 +12,18 @@
 // outcome_ of the reference (connect_four.h:58-63) is cached in bits 62-63 of the key, exactly as the
 // reference caches it in `outcome_`: a step then costs ONE line test (for the stone just dropped) instead of
 // re-deriving the outcome before and after.  Larger boards derive it on load.
+// Two instantiations of one source: ConnectFourCore<true> is the default board (6x7, four in a row) with every size a
+// compile-time constant, so the kernels' shifts by rows+1, rows and columns are immediates instead of 64-bit shifts by a
+// run-time amount (the batched ApplyAction of the default board is an HBM stream whose integer work otherwise shows);
+// ConnectFourCore<false> (ConnectFourRules) reads the sizes from the configuration and serves every other board and the
+// host tools.
 #pragma once
 #include "common.cuh"
 
 namespace b2s {
 
-struct ConnectFourRules {
+template <bool kStd>
+struct ConnectFourCore {
   static constexpr int kGameId = B2S_CONNECT_FOUR;
   typedef uint4 Chunk;                 // the lane blob: {x, o}
   typedef u64 Packed;                  // a lane in a device batch: the key
@@ -31,6 +37,7 @@ struct ConnectFourRules {
   static constexpr int kIlp = 4;      // lanes per thread in the streaming kernels (8 was measured slower with 8-byte lanes: k_step_fused then needs 58 registers)
   static constexpr int kMinBlocks = 6;   // <= 42 registers (capping k_apply at 32 registers to fit the 1M-lane grid in one wave spills and was measured 20 % slower)
   static constexpr bool kHasInfoState = false;
+  static constexpr int kStdRows = 6, kStdCols = 7, kStdK = 4;   // connect_four.h:45-50 defaults
 
   struct Cfg {
     int rows, cols, k, ego;
@@ -52,6 +59,12 @@ struct ConnectFourRules {
   // as outcome ^ 2 so that "unknown" is all-zero.  outcome: 0 = player 0 won, 1 = player 1 won, 2 = unknown,
   // 3 = draw (connect_four.h:58-63).
   struct S { u64 x, o; };   // player 0 ("x", kCross) / player 1 ("o", kNought) stones
+  // the sizes as the device code reads them: constants on the default board
+  __host__ __device__ static __forceinline__ int ROWS(const Cfg& c) { return kStd ? kStdRows : c.rows; }
+  __host__ __device__ static __forceinline__ int COLS(const Cfg& c) { return kStd ? kStdCols : c.cols; }
+  __host__ __device__ static __forceinline__ int H1(const Cfg& c) { return kStd ? kStdRows + 1 : c.h1; }
+  __host__ __device__ static __forceinline__ int K(const Cfg& c) { return kStd ? kStdK : c.k; }
+  __host__ __device__ static __forceinline__ bool META(const Cfg& c) { return kStd ? true : c.meta != 0; }
 
   static __host__ const char* make_cfg(const b2s_params& p, Cfg& c, b2s_game_info& gi) {
     c.rows = p.rows >= 0 ? p.rows : 6;            // connect_four.h:45-50 defaults
@@ -61,6 +74,7 @@ struct ConnectFourRules {
     if (c.rows < 1 || c.cols < 1 || c.k < 1) return "connect_four: rows, columns, x_in_row must be positive";
     if ((c.rows + 1) * c.cols > 64 || c.cols > 32)
       return "connect_four: (rows+1)*columns must fit 64 bits for the device path";
+    if (kStd && (c.rows != kStdRows || c.cols != kStdCols || c.k != kStdK)) return "connect_four: not the default board";
     c.h1 = c.rows + 1;
     c.meta = (c.rows + 1) * c.cols <= 62 ? 1 : 0;
     c.top = 0; c.board = 0; c.bottom = 0;
@@ -153,17 +167,17 @@ struct ConnectFourRules {
   }
 
   __device__ static __forceinline__ bool has_line(u64 b, const Cfg& c) {
-    if (c.k == 4) {
-      const int d1 = c.h1, d2 = c.h1 + 1, d3 = c.h1 - 1;
+    if (K(c) == 4) {
+      const int d1 = H1(c), d2 = H1(c) + 1, d3 = H1(c) - 1;
       u64 m1 = b & (b >> 1), m2 = b & (b >> d1), m3 = b & (b >> d2), m4 = b & (b >> d3);
       u64 any = (m1 & (m1 >> 2)) | (m2 & (m2 >> (2 * d1))) | (m3 & (m3 >> (2 * d2))) | (m4 & (m4 >> (2 * d3)));
       return any != 0;
     }
-    const int d[4] = {1, c.h1, c.h1 + 1, c.h1 - 1};
+    const int d[4] = {1, H1(c), H1(c) + 1, H1(c) - 1};
     for (int j = 0; j < 4; ++j) {
       u64 m = b;
       bool ok = true;
-      for (int i = 1; i < c.k; ++i) {
+      for (int i = 1; i < K(c); ++i) {
         int sh = i * d[j];
         if (sh >= 64) { ok = false; break; }
         m &= b >> sh;
@@ -172,7 +186,7 @@ struct ConnectFourRules {
     }
     return false;
   }
-  __host__ __device__ static __forceinline__ u64 xs(const S& s, const Cfg& c) { return c.meta ? (s.x & ~(3ull << 62)) : s.x; }
+  __host__ __device__ static __forceinline__ u64 xs(const S& s, const Cfg& c) { return META(c) ? (s.x & ~(3ull << 62)) : s.x; }
   __device__ static __forceinline__ int mover(const S& s, const Cfg& c) { return __popcll(xs(s, c) | s.o) & 1; }
   __device__ static __forceinline__ int derive_outcome(u64 x, u64 o, const Cfg& c) {
     int last = 1 - (__popcll(x | o) & 1);            // only the player who just moved can have completed a line
@@ -181,7 +195,7 @@ struct ConnectFourRules {
     return 2;
   }
   __device__ static __forceinline__ int outcome(const S& s, const Cfg& c) {
-    return c.meta ? ((int)(s.x >> 62) ^ 2) : derive_outcome(s.x, s.o, c);
+    return META(c) ? ((int)(s.x >> 62) ^ 2) : derive_outcome(s.x, s.o, c);
   }
 
   __host__ __device__ static __forceinline__ void load(S& s, const Ctx& ctx, long long i) {
@@ -199,13 +213,13 @@ struct ConnectFourRules {
     f |= (f >> 1) & c.fill[0];
     f |= (f >> 2) & c.fill[1];
     f |= (f >> 4) & c.fill[2];
-    if (c.h1 > 8) {
+    if (H1(c) > 8) {
       f |= (f >> 8) & c.fill[3];
       f |= (f >> 16) & c.fill[4];
       f |= (f >> 32) & c.fill[5];
     }
     const u64 occ = (f >> 1) & c.fill[0];           // the rows below each marker
-    s.x = key & (occ | (c.meta ? 3ull << 62 : 0ull));
+    s.x = key & (occ | (META(c) ? 3ull << 62 : 0ull));
     s.o = occ & ~key;
   }
   // occ + bottom carries every column's stone stack into its marker bit
@@ -227,16 +241,16 @@ struct ConnectFourRules {
     u64 free_top = ~(xs(s, c) | s.o) & c.top;
     if (c.gather) {
       u32 lo = (u32)free_top, hi = (u32)(free_top >> 32);
-      u32 out = (((lo >> (c.rows - 1)) * c.gmul_lo) >> c.gsh_lo) & ((1u << c.cols_lo) - 1);
-      if (c.cols_lo < c.cols) {
-        int first_hi = c.cols_lo * c.h1 + c.rows - 1 - 32;
-        out |= ((((hi >> first_hi) * c.gmul_hi) >> c.gsh_hi) & ((1u << (c.cols - c.cols_lo)) - 1)) << c.cols_lo;
+      u32 out = (((lo >> (ROWS(c) - 1)) * c.gmul_lo) >> c.gsh_lo) & ((1u << c.cols_lo) - 1);
+      if (c.cols_lo < COLS(c)) {
+        int first_hi = c.cols_lo * H1(c) + ROWS(c) - 1 - 32;
+        out |= ((((hi >> first_hi) * c.gmul_hi) >> c.gsh_hi) & ((1u << (COLS(c) - c.cols_lo)) - 1)) << c.cols_lo;
       }
       m[0] = out;
       return;
     }
     u32 out = 0;
-    for (int col = 0; col < c.cols; ++col) out |= (u32)((free_top >> (col * c.h1 + c.rows - 1)) & 1ull) << col;
+    for (int col = 0; col < COLS(c); ++col) out |= (u32)((free_top >> (col * H1(c) + ROWS(c) - 1)) & 1ull) << col;
     m[0] = out;
   }
   __device__ static __forceinline__ void legal(const S& s, const Cfg& c, u32* m) {
@@ -245,17 +259,17 @@ struct ConnectFourRules {
   }
   // Apply to a NON-terminal state; false = illegal (state untouched).
   __device__ static __forceinline__ bool apply(S& s, int a, const Cfg& c, const Ctx&, long long) {
-    if (a < 0 || a >= c.cols) return false;
+    if (a < 0 || a >= COLS(c)) return false;
     u64 x = xs(s, c);
     u64 occ = x | s.o;
-    int base = a * c.h1;
-    if ((occ >> (base + c.rows - 1)) & 1ull) return false;
-    u64 colmask = ((1ull << c.rows) - 1) << base;
+    int base = a * H1(c);
+    if ((occ >> (base + ROWS(c) - 1)) & 1ull) return false;
+    u64 colmask = ((1ull << ROWS(c)) - 1) << base;
     u64 bit = (occ & colmask) + (1ull << base);
     int mv = __popcll(occ) & 1;
     u64 mine = (mv == 0 ? x : s.o) | bit;
     if (mv == 0) x = mine; else s.o = mine;
-    if (c.meta) {
+    if (META(c)) {
       // outcome_ after the move (connect_four.cc:139-143): a line for the mover, else a full board
       int oc = has_line(mine, c) ? mv : (((occ | bit) & c.top) == c.top ? 3 : 2);
       x |= (u64)(oc ^ 2) << 62;
@@ -280,19 +294,21 @@ struct ConnectFourRules {
     if (c.rgather) {
       u64 colbits = c.board & ~(c.board << 1);             // bit c*h1 of every column
       int e = 0;
+#pragma unroll
       for (int pl = 0; pl < 3; ++pl)
-        for (int r = 0; r < c.rows; ++r, e += c.cols) {
+        for (int r = 0; r < ROWS(c); ++r, e += COLS(c)) {
           u64 row = (u64)row_gather_eval(c, (planes[pl] >> r) & colbits);
           p.w[e >> 6] |= row << (e & 63);
-          if ((e & 63) + c.cols > 64) p.w[(e >> 6) + 1] |= row >> (64 - (e & 63));
+          if ((e & 63) + COLS(c) > 64) p.w[(e >> 6) + 1] |= row >> (64 - (e & 63));
         }
       return;
     }
     int e = 0;
+#pragma unroll
     for (int pl = 0; pl < 3; ++pl)
-      for (int r = 0; r < c.rows; ++r)
-        for (int col = 0; col < c.cols; ++col, ++e) {
-          u64 bit = (planes[pl] >> (col * c.h1 + r)) & 1ull;
+      for (int r = 0; r < ROWS(c); ++r)
+        for (int col = 0; col < COLS(c); ++col, ++e) {
+          u64 bit = (planes[pl] >> (col * H1(c) + r)) & 1ull;
           p.w[e >> 6] |= bit << (e & 63);
         }
   }
@@ -300,5 +316,8 @@ struct ConnectFourRules {
     return (float)((p.w[e >> 6] >> (e & 63)) & 1ull);
   }
 };
+
+typedef ConnectFourCore<false> ConnectFourRules;   // every board; the host tools' core
+typedef ConnectFourCore<true> ConnectFourStdRules;  // the default 6x7 board, four in a row
 
 }  // namespace b2s

@@ -1,6 +1,8 @@
 // Microbenchmark (development tool, not part of the library): connect_four ApplyAction kernel variants on
 // rotating 1M-state batches inside a CUDA graph, to pick ILP / block size / launch attributes: the earlier 16-byte
-// two-board lanes ({x, o}) and the library's 8-byte lanes.
+// two-board lanes ({x, o}), the library's 8-byte lanes and 7-byte lanes in 32-lane tiles (measured, not adopted: DESIGN §3),
+// each beside a pure copy kernel that moves the same bytes per lane (the ceiling an ApplyAction of that lane format is judged
+// against).
 // nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o apply_variants apply_variants.cu
 #include <cstdio>
 #include <cstdlib>
@@ -94,19 +96,21 @@ __global__ void __launch_bounds__(BLOCK) k_apply_gs(ulonglong2* st, const int* _
 // outcome sits in bits 62-63 as outcome ^ 2 (0 = game running).
 constexpr u64 BOTTOM = 0x40810204081ull;                                  // bit col*7
 constexpr u64 L1 = BOTTOM * 0x3f, L2 = BOTTOM * 0x1f, L4 = BOTTOM * 0x7;   // in-column rows < 6, < 5, < 3
+// MS: bit of the cached outcome (62: 8-byte key, 54: 7-byte key)
+template <int MS = 62>
 __device__ __forceinline__ bool step8(u64& key, int a, unsigned long long* err) {
   if (a == -1) return false;
   u64 s = key;
   s |= (s >> 1) & L1; s |= (s >> 2) & L2; s |= (s >> 4) & L4;          // every column filled up to its marker
   const u64 occ = (s >> 1) & L1;
   u64 x = key & occ, o = occ & ~key;
-  if ((key >> 62) || a < 0 || a >= 7 || ((occ >> (a * 7 + 5)) & 1)) { atomicAdd(err, 1ull); return false; }
+  if ((key >> MS) || a < 0 || a >= 7 || ((occ >> (a * 7 + 5)) & 1)) { atomicAdd(err, 1ull); return false; }
   const u64 bit = (occ & (0x3full << (a * 7))) + (1ull << (a * 7));
   const int mover = __popcll(occ) & 1;
   const u64 mine = (mover ? o : x) | bit;
   if (mover == 0) x = mine; else o = mine;
   const int oc = has_line(mine) ? mover : (((occ | bit) & (BOTTOM << 5)) == (BOTTOM << 5) ? 3 : 2);
-  key = x | ((x | o) + BOTTOM) | ((u64)(oc ^ 2) << 62);
+  key = x | ((x | o) + BOTTOM) | ((u64)(oc ^ 2) << MS);
   return true;
 }
 
@@ -144,6 +148,71 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_apply8_pair(u64* st, const int*
   }
 }
 
+// 7-byte keys in 32-lane tiles (common.cuh LaneTiles<4, 2, 1>): bytes 0-3 of the tile's 32 lanes, then bytes 4-5, then byte
+// 6, 224 B per tile; the lanes of thread j are 8 j tiles past its first lane, at the same slot
+__device__ __forceinline__ u64 tile7_get(const unsigned char* t, int slot) {
+  return (u64)reinterpret_cast<const unsigned*>(t)[slot] | (u64)reinterpret_cast<const unsigned short*>(t + 128)[slot] << 32 |
+         (u64)t[192 + slot] << 48;
+}
+__device__ __forceinline__ void tile7_set(unsigned char* t, int slot, u64 key) {
+  reinterpret_cast<unsigned*>(t)[slot] = (unsigned)key;
+  reinterpret_cast<unsigned short*>(t + 128)[slot] = (unsigned short)(key >> 32);
+  t[192 + slot] = (unsigned char)(key >> 48);
+}
+template <int ILP, int BLOCK, int MINB>
+__global__ void __launch_bounds__(BLOCK, MINB) k_apply7(unsigned char* st, const int* __restrict__ act, long long n, unsigned long long* err) {
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  long long base = (long long)blockIdx.x * (BLOCK * ILP) + threadIdx.x;
+  unsigned char* t0 = st + (base >> 5) * 224;
+  const int slot = threadIdx.x & 31;
+  int a[ILP]; u64 s[ILP];
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) { long long i = base + (long long)j * BLOCK; a[j] = -1; if (i < n) { a[j] = __ldg(act + i); s[j] = tile7_get(t0 + j * (BLOCK / 32) * 224, slot); } }
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) if (step8<54>(s[j], a[j], err)) tile7_set(t0 + j * (BLOCK / 32) * 224, slot, s[j]);
+}
+
+// pure copies of the same traffic: lane state in, action in, state + action out (no game logic) — 8-byte lanes: 12 R / 8 W
+// = 20 B, 7-byte tiled lanes: 11 R / 7 W = 18 B
+template <int ILP, int BLOCK, int MINB>
+__global__ void __launch_bounds__(BLOCK, MINB) k_copy8(u64* st, const int* __restrict__ act, long long n, unsigned long long*) {
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  long long base = (long long)blockIdx.x * (BLOCK * ILP) + threadIdx.x;
+  int a[ILP]; u64 s[ILP];
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) { long long i = base + (long long)j * BLOCK; a[j] = -1; if (i < n) { a[j] = __ldg(act + i); s[j] = st[i]; } }
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) { long long i = base + (long long)j * BLOCK; if (a[j] != -1) st[i] = s[j] + (u64)a[j]; }
+}
+template <int ILP, int BLOCK, int MINB>
+__global__ void __launch_bounds__(BLOCK, MINB) k_copy7(unsigned char* st, const int* __restrict__ act, long long n, unsigned long long*) {
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  long long base = (long long)blockIdx.x * (BLOCK * ILP) + threadIdx.x;
+  unsigned char* t0 = st + (base >> 5) * 224;
+  const int slot = threadIdx.x & 31;
+  int a[ILP]; u64 s[ILP];
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) { long long i = base + (long long)j * BLOCK; a[j] = -1; if (i < n) { a[j] = __ldg(act + i); s[j] = tile7_get(t0 + j * (BLOCK / 32) * 224, slot); } }
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) if (a[j] != -1) tile7_set(t0 + j * (BLOCK / 32) * 224, slot, s[j] + (u64)a[j]);
+}
+
+template <int ILP, int BLOCK, int MINB, int KIND>   // KIND 2: apply7, 3: copy8, 4: copy7
+void launch_k(void* st, const int* act, long long n, unsigned long long* err, cudaStream_t s) {
+  unsigned grid = (unsigned)((n + (long long)BLOCK * ILP - 1) / ((long long)BLOCK * ILP));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(BLOCK); cfg.stream = s;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  if (KIND == 2) CK(cudaLaunchKernelEx(&cfg, k_apply7<ILP, BLOCK, MINB>, (unsigned char*)st, act, n, err));
+  else if (KIND == 3) CK(cudaLaunchKernelEx(&cfg, k_copy8<ILP, BLOCK, MINB>, (u64*)st, act, n, err));
+  else CK(cudaLaunchKernelEx(&cfg, k_copy7<ILP, BLOCK, MINB>, (unsigned char*)st, act, n, err));
+}
+
 template <int ILP, int BLOCK, int MINB, bool PAIR>
 void launch8(void* st, const int* act, long long n, unsigned long long* err, cudaStream_t s) {
   long long units = PAIR ? n / 2 : n;
@@ -158,7 +227,7 @@ void launch8(void* st, const int* act, long long n, unsigned long long* err, cud
 }
 
 struct Variant { const char* name; void (*launch)(ulonglong2*, const int*, long long, unsigned long long*, cudaStream_t); };
-struct Variant8 { const char* name; void (*launch)(void*, const int*, long long, unsigned long long*, cudaStream_t); };
+struct Variant8 { const char* name; void (*launch)(void*, const int*, long long, unsigned long long*, cudaStream_t); double bytes = 20; };
 
 template <int ILP, int BLOCK, bool PDL>
 void launch_v(ulonglong2* st, const int* act, long long n, unsigned long long* err, cudaStream_t s) {
@@ -237,12 +306,14 @@ int main(int argc, char** argv) {
     {"c8_ilp4_b512_m1", launch8<4, 512, 1, false>},
     {"c8_pair2_b256_m6", launch8<2, 256, 6, true>}, {"c8_pair4_b256_m1", launch8<4, 256, 1, true>},
     {"c8_pair4_b256_m6", launch8<4, 256, 6, true>},
+    {"copy8_ilp4_b256_m6", launch_k<4, 256, 6, 3>, 20},
+    {"c7_ilp4_b256_m6", launch_k<4, 256, 6, 2>, 18}, {"copy7_ilp4_b256_m6", launch_k<4, 256, 6, 4>, 18},
   };
   cudaStream_t s2; CK(cudaStreamCreate(&s2));
   cudaEvent_t fork, join; CK(cudaEventCreateWithFlags(&fork, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&join, cudaEventDisableTiming));
   for (int chains = 1; chains <= 2; ++chains) {
     for (auto& v : v8) {
-      for (int k = 0; k < slots; ++k) CK(cudaMemsetAsync(st[k], 0, n * 8, s));    // all-zero keys decode to the empty board
+      for (int k = 0; k < slots; ++k) CK(cudaMemsetAsync(st[k], 0, n * 8, s));    // all-zero keys decode to the empty board (n * 8 bytes hold n tiled 7-byte lanes for n % 32 == 0)
       cudaGraph_t g; cudaGraphExec_t ge;
       CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeGlobal));
       if (chains == 2) { CK(cudaEventRecord(fork, s)); CK(cudaStreamWaitEvent(s2, fork, 0)); }
@@ -258,7 +329,7 @@ int main(int argc, char** argv) {
         float ms; CK(cudaEventElapsedTime(&ms, e0, e1)); if (ms < best) best = ms;
       }
       double us = best * 1e3 / K;
-      printf("%-20s chains=%d n=%lld  %.2f us/step  %.1f GB/s (20 B/step)  %.3e steps/s\n", v.name, chains, n, us, 20.0 * n / us / 1e3, n / us * 1e6);
+      printf("%-20s chains=%d n=%lld  %.2f us/step  %.1f GB/s (%.0f B/step)  %.3e steps/s\n", v.name, chains, n, us, v.bytes * n / us / 1e3, v.bytes, n / us * 1e6);
       CK(cudaGraphExecDestroy(ge)); CK(cudaGraphDestroy(g));
     }
   }
