@@ -756,8 +756,16 @@ class CFRSolver:
         self.load_table(r, c, p, iteration=parsed["iteration"])
         return parsed
 
+    _has_current_policy = True
+
+    def _require_current_policy(self):
+        if not self._has_current_policy:
+            raise B2SError("%s keeps no current policy: use the average policy" % type(self).__name__)
+
     def nash_conv(self, average=True):
         """algorithms::NashConv (tabular_exploitability.cc) of the average (default) or current policy, on the device."""
+        if not average:
+            self._require_current_policy()
         nc = C.c_double()
         vals = (C.c_double * 4)()
         check(lib().b2s_cfr_nash_conv(self._h, int(bool(average)), C.byref(nc), vals, None))
@@ -768,6 +776,8 @@ class CFRSolver:
         """TabularBestResponse of each player against the other's average (default) / current policy, on the device:
         (actions, values) with actions[I] = the legal action chosen at information state I (table() order; first maximum, as
         best_response.cc:194-228) and values = [BR value p0, BR value p1, on-policy value p0, on-policy value p1]."""
+        if not average:
+            self._require_current_policy()
         i = self._info
         idx = np.empty(i.num_infosets, dtype=np.int32)
         vals = (C.c_double * 4)()
@@ -781,6 +791,7 @@ class CFRSolver:
 
     def current_policy(self):
         """CFRCurrentPolicy (cfr.cc:139-165): {key bytes: [(action, prob)]} from the current-policy table."""
+        self._require_current_policy()
         t = self.table()
         return {t["keys"][k].tobytes(): list(zip(t["legal_actions"][t["offsets"][k]:t["offsets"][k + 1]].tolist(),
                                                  t["cur_policy"][t["offsets"][k]:t["offsets"][k + 1]].tolist()))
@@ -819,7 +830,11 @@ class CFRSolver:
 class ExternalSamplingMCCFRSolver(CFRSolver):
     """Mirror of pyspiel.ExternalSamplingMCCFRSolver(game, seed, avg_type=kSimple)
     (algorithms/external_sampling_mccfr.h:55-110) with device-resident tables.  `traversals_per_update` independent
-    traversals run in parallel per (iteration, traverser) phase against frozen tables; 1 = the reference's algorithm."""
+    traversals run in parallel per (iteration, traverser) phase against frozen tables; 1 = the reference's algorithm.
+    Like the reference, it has no current policy: simple averaging runs regret matching on a copy and never writes the
+    current-policy table, so nash_conv / best_response(average=False) and current_policy() raise B2SError."""
+
+    _has_current_policy = False
 
     def __init__(self, game, seed=0, traversals_per_update=1, full_average=False):
         """full_average = AverageType::kFull (external_sampling_mccfr.h:53-54) instead of the default kSimple."""
@@ -839,7 +854,10 @@ class ExternalSamplingMCCFRSolver(CFRSolver):
 class OutcomeSamplingMCCFRSolver(CFRSolver):
     """Mirror of pyspiel.OutcomeSamplingMCCFRSolver(game, epsilon, seed) (algorithms/outcome_sampling_mccfr.h:40-66; default
     uniform policy, no baseline) with device-resident tables.  `trajectories_per_update` independent episodes run in parallel
-    per (iteration, player) phase against frozen tables; 1 = the reference's algorithm."""
+    per (iteration, player) phase against frozen tables; 1 = the reference's algorithm.  No current policy, as for
+    ExternalSamplingMCCFRSolver."""
+
+    _has_current_policy = False
 
     def __init__(self, game, epsilon=0.6, seed=0, trajectories_per_update=1):
         super().__init__(game, _mccfr_tables=True)
