@@ -358,7 +358,8 @@ int  b2s_cfr_delta_buffer(void* solver, double** delta_d);
 int  b2s_cfr_delta_count(void* solver, int64_t* count);
 /* In-library exchange (NCCL over NVLink; NCCL is resolved with dlopen, the copy already loaded in the process wins).
  * b2s_nccl_unique_id: 128-byte ncclUniqueId created on one rank, to be handed to all ranks by the caller's own means.
- * b2s_cfr_comm_init creates a communicator owned by the solver; b2s_cfr_comm_adopt uses the caller's ncclComm_t.
+ * b2s_cfr_comm_init creates a communicator owned by the solver; b2s_cfr_comm_adopt uses the caller's ncclComm_t, which
+ * must be a blocking one (the library does not poll ncclInProgress) and which the solver never destroys.
  * b2s_cfr_iterate_sharded: `iters` x CFRSolverBase::EvaluateAndUpdatePolicy (cfr.cc:263-282) with traverse -> ncclAllReduce
  * -> apply enqueued back to back on a solver-owned stream (ordered after / before `stream`), 16 iterations per CUDA graph
  * launch — no host code between the steps.  Collective: every rank must make the same call.

@@ -91,7 +91,6 @@ class DistributedCFRSolver:
         import torch.distributed as dist
         self.solver = CFRSolver(game, linear_averaging, regret_matching_plus)
         self.rank, self.world = world()
-        self.iteration = 0
         ptr, cnt = C.c_void_p(), C.c_int64()
         check(lib().b2s_cfr_delta_buffer(self.solver._h, C.byref(ptr)))
         check(lib().b2s_cfr_delta_count(self.solver._h, C.byref(cnt)))
@@ -108,20 +107,24 @@ class DistributedCFRSolver:
                 dist.broadcast_object_list(box, src=0)
             check(lib().b2s_cfr_comm_init(self.solver._h, box[0], self.rank, self.world))
 
+    @property
+    def iteration(self):
+        """The wrapped solver's iteration counter (it moves with single-GPU calls and load_table too)."""
+        return self.solver.info().iteration
+
     def evaluate_and_update_policy(self, iterations=1):
         L, h = lib(), self.solver._h
         st = C.c_void_p(torch.cuda.current_stream(self.delta.device).cuda_stream)
         if self.in_library:
             check(L.b2s_cfr_iterate_sharded(h, int(iterations), st))
-            self.iteration += int(iterations)
             return
         for _ in range(int(iterations)):
-            self.iteration += 1
+            iteration = self.iteration + 1
             for player in (0, 1):
-                check(L.b2s_cfr_traverse_shard(h, player, self.iteration, self.rank, self.world, st))
+                check(L.b2s_cfr_traverse_shard(h, player, iteration, self.rank, self.world, st))
                 allreduce_stats(self.delta)
                 check(L.b2s_cfr_apply_deltas(h, st))
-        check(L.b2s_cfr_set_iteration(h, self.iteration))
+            check(L.b2s_cfr_set_iteration(h, iteration))
 
     def allreduce_seconds(self, count=200):
         """Device seconds of `count` back-to-back all-reduces of the contribution buffer (latency floor of the exchange)."""

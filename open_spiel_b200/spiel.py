@@ -709,10 +709,13 @@ class CFRSolver:
         check(lib().b2s_cfr_info_get(self._h, C.byref(i)))
         return i
 
+    def _stream(self):
+        """torch's current stream on the solver's device: every call below is ordered on it, as torch's own work is."""
+        return C.c_void_p(torch.cuda.current_stream(torch.device("cuda", self.game.device)).cuda_stream)
+
     def evaluate_and_update_policy(self, iterations=1):
         """CFRSolverBase::EvaluateAndUpdatePolicy (cfr.cc:263-282), `iterations` times in one kernel launch."""
-        st = C.c_void_p(torch.cuda.current_stream(torch.device("cuda", self.game.device)).cuda_stream)
-        check(lib().b2s_cfr_iterate(self._h, int(iterations), st))
+        check(lib().b2s_cfr_iterate(self._h, int(iterations), self._stream()))
 
     def table(self):
         """The info-state table as numpy arrays: dict(regrets, cum_policy, cur_policy, offsets, legal_actions,
@@ -724,14 +727,14 @@ class CFRSolver:
                "players": np.empty(I, dtype=np.int32), "keys": np.empty((I, T), dtype=np.float32)}
         p = lambda a: a.ctypes.data_as(C.c_void_p)   # noqa: E731
         check(lib().b2s_cfr_export(self._h, p(out["regrets"]), p(out["cum_policy"]), p(out["cur_policy"]),
-                                   p(out["offsets"]), p(out["legal_actions"]), p(out["players"]), p(out["keys"]), None))
+                                   p(out["offsets"]), p(out["legal_actions"]), p(out["players"]), p(out["keys"]), self._stream()))
         return out
 
     def load_table(self, regrets=None, cum_policy=None, cur_policy=None, iteration=-1):
         p = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float64).ctypes.data_as(C.c_void_p)   # noqa: E731
         keep = [np.ascontiguousarray(a, dtype=np.float64) if a is not None else None for a in (regrets, cum_policy, cur_policy)]
         check(lib().b2s_cfr_import(self._h, *[None if a is None else a.ctypes.data_as(C.c_void_p) for a in keep],
-                                   int(iteration), None))
+                                   int(iteration), self._stream()))
 
     def table_pointers(self):
         r, c, u = C.c_void_p(), C.c_void_p(), C.c_void_p()
@@ -768,7 +771,7 @@ class CFRSolver:
             self._require_current_policy()
         nc = C.c_double()
         vals = (C.c_double * 4)()
-        check(lib().b2s_cfr_nash_conv(self._h, int(bool(average)), C.byref(nc), vals, None))
+        check(lib().b2s_cfr_nash_conv(self._h, int(bool(average)), C.byref(nc), vals, self._stream()))
         self.last_values = list(vals)
         return nc.value
 
@@ -781,7 +784,7 @@ class CFRSolver:
         i = self._info
         idx = np.empty(i.num_infosets, dtype=np.int32)
         vals = (C.c_double * 4)()
-        check(lib().b2s_cfr_best_response(self._h, int(bool(average)), idx.ctypes.data_as(C.c_void_p), vals, None))
+        check(lib().b2s_cfr_best_response(self._h, int(bool(average)), idx.ctypes.data_as(C.c_void_p), vals, self._stream()))
         t = self.table()
         return t["legal_actions"][t["offsets"][:-1] + idx], list(vals)
 
@@ -843,9 +846,8 @@ class ExternalSamplingMCCFRSolver(CFRSolver):
 
     def run_iteration(self, iterations=1):
         """ExternalSamplingMCCFRSolver::RunIteration (external_sampling_mccfr.cc:71-80), `iterations` times."""
-        st = C.c_void_p(torch.cuda.current_stream(torch.device("cuda", self.game.device)).cuda_stream)
         check(lib().b2s_mccfr_external_iterate_ex(self._h, int(iterations), self.traversals_per_update, self.seed,
-                                                  1 if self.full_average else 0, st))
+                                                  1 if self.full_average else 0, self._stream()))
 
     def evaluate_and_update_policy(self, iterations=1):
         raise B2SError("ExternalSamplingMCCFRSolver: use run_iteration()")
@@ -865,8 +867,7 @@ class OutcomeSamplingMCCFRSolver(CFRSolver):
 
     def run_iteration(self, iterations=1):
         """OutcomeSamplingMCCFRSolver::RunIteration (outcome_sampling_mccfr.cc:60-67), `iterations` times."""
-        st = C.c_void_p(torch.cuda.current_stream(torch.device("cuda", self.game.device)).cuda_stream)
-        check(lib().b2s_mccfr_outcome_iterate(self._h, int(iterations), self.trajectories_per_update, self.seed, self.epsilon, st))
+        check(lib().b2s_mccfr_outcome_iterate(self._h, int(iterations), self.trajectories_per_update, self.seed, self.epsilon, self._stream()))
 
     def evaluate_and_update_policy(self, iterations=1):
         raise B2SError("OutcomeSamplingMCCFRSolver: use run_iteration()")

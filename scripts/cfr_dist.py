@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
 """Multi-GPU CFR exchange, measured (run under torchrun, one rank per GPU):
-  * exactness: in-library NCCL-sharded Leduc CFR vs the single-GPU solver at 1k / 10k / 100k iterations (max |delta| of
-    cumulative regrets, cumulative policy, current policy; expected 0 — bit-identical)
+  * exactness: in-library NCCL-sharded Leduc CFR and CFR+ vs the single-GPU solver at 1k / 10k / 100k iterations (max
+    |delta| of cumulative regrets, cumulative policy, current policy; expected 0 — bit-identical).  CFR+'s linear averaging
+    weights every average-policy increment by the iteration number, which the sharded loop keeps in a device counter
   * throughput: iterations/s of the sharded loop (16 iterations per CUDA-graph launch, no host code between the steps)
     vs the single-GPU persistent kernel
   * latency floor: device time of one ncclAllReduce of the contribution buffer (2C doubles), two of which every
@@ -26,30 +27,37 @@ torch.cuda.set_device(local)
 dev = torch.device("cuda", local)
 dist.init_process_group("nccl", device_id=dev)
 game = b2.Game("leduc_poker", device=local)
-sharded = parallel.DistributedCFRSolver(game)
-single = b2.CFRSolver(game)
-res = {"world": world, "game": "leduc_poker", "contribution_doubles": int(sharded.delta.numel()), "checkpoints": []}
+VARIANTS = {"cfr": (False, False), "cfr_plus": (True, True)}      # (linear averaging, regret matching+)
+solvers = {v: (parallel.DistributedCFRSolver(game, la, rm, in_library=True), b2.CFRSolver(game, la, rm))
+           for v, (la, rm) in VARIANTS.items()}
+sharded = solvers["cfr"][0]
+res = {"world": world, "game": "leduc_poker", "contribution_doubles": int(sharded.delta.numel()),
+       "checkpoints": {v: [] for v in VARIANTS}}
 done = 0
 for target in (1000, 10000, 100000):
-    torch.cuda.synchronize(); dist.barrier()
-    t0 = time.perf_counter()
-    sharded.evaluate_and_update_policy(target - done)
-    torch.cuda.synchronize()
-    t_sh = time.perf_counter() - t0
-    t0 = time.perf_counter()
-    single.evaluate_and_update_policy(target - done)
-    torch.cuda.synchronize()
-    t_1 = time.perf_counter() - t0
-    ts, t1 = sharded.table(), single.table()
-    err = {f: float(np.abs(ts[f] - t1[f]).max()) for f in ("regrets", "cum_policy", "cur_policy")}
-    res["checkpoints"].append({"iterations": target, "max_abs_diff": err, "bit_identical": all(np.array_equal(ts[f], t1[f]) for f in err),
-                               "sharded_iters_per_s": (target - done) / t_sh, "single_gpu_iters_per_s": (target - done) / t_1})
+    for v, (sh, single) in solvers.items():
+        torch.cuda.synchronize(); dist.barrier()
+        t0 = time.perf_counter()
+        sh.evaluate_and_update_policy(target - done)
+        torch.cuda.synchronize()
+        t_sh = time.perf_counter() - t0
+        t0 = time.perf_counter()
+        single.evaluate_and_update_policy(target - done)
+        torch.cuda.synchronize()
+        t_1 = time.perf_counter() - t0
+        ts, t1 = sh.table(), single.table()
+        err = {f: float(np.abs(ts[f] - t1[f]).max()) for f in ("regrets", "cum_policy", "cur_policy")}
+        res["checkpoints"][v].append({"iterations": target, "max_abs_diff": err,
+                                      "bit_identical": all(np.array_equal(ts[f], t1[f]) for f in err),
+                                      "iteration_counters": [sh.iteration, single.info().iteration],
+                                      "sharded_iters_per_s": (target - done) / t_sh, "single_gpu_iters_per_s": (target - done) / t_1})
     done = target
-res["exploitability_sharded"] = sharded.solver.exploitability()
-res["exploitability_single"] = single.exploitability()
+for v, (sh, single) in solvers.items():
+    res["exploitability_sharded_" + v] = sh.solver.exploitability()
+    res["exploitability_single_" + v] = single.exploitability()
 secs = sharded.allreduce_seconds(400)
 res["allreduce_us"] = secs / 400 * 1e6
-best = res["checkpoints"][-1]
+best = res["checkpoints"]["cfr"][-1]
 res["iteration_us_single_gpu"] = 1e6 / best["single_gpu_iters_per_s"]
 res["iteration_us_sharded"] = 1e6 / best["sharded_iters_per_s"]
 res["floor_note"] = ("one iteration needs 2 all-reduces = %.1f us of exchange latency on top of two traversals whose level passes are "
