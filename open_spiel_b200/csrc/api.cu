@@ -551,7 +551,7 @@ int b2s_broadcast_state(void* dst_batch, int64_t dst_begin, int64_t count, void*
       memcmp(&D->info, &S->info, sizeof(b2s_game_info)) != 0)
     return fail("broadcast: batches differ in game/params/device");
   if (dst_begin < 0 || count < 0 || dst_begin + count > D->cap || src < 0 || src >= S->cap) return fail("broadcast: range");
-  D->ops->broadcast(D->ctx(), dst_begin, count, S->ctx(), src, (cudaStream_t)stream);
+  D->ops->copy(D->ctx(), dst_begin, S->ctx(), src, 0, count, (cudaStream_t)stream);
   return post();
 }
 
@@ -564,7 +564,7 @@ int b2s_copy_states(void* dst_batch, int64_t dst_begin, void* src_batch, int64_t
     return fail("copy: batches differ in game/params/device");
   if (dst_begin < 0 || src_begin < 0 || count < 0 || dst_begin + count > D->cap || src_begin + count > S->cap)
     return fail("copy: range");
-  D->ops->copy(D->ctx(), dst_begin, S->ctx(), src_begin, count, (cudaStream_t)stream);
+  D->ops->copy(D->ctx(), dst_begin, S->ctx(), src_begin, 1, count, (cudaStream_t)stream);
   return post();
 }
 

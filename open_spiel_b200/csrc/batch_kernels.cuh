@@ -21,18 +21,68 @@ extern long long g_launches;   // api.cu
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-template <typename... KArgs, typename... Args>
-inline void launch_pdl(void (*kernel)(KArgs...), unsigned grid, cudaStream_t st, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(kBlock);
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+inline unsigned grid_for(long long n, int ilp = 1) { return (unsigned)((n + (long long)kBlock * ilp - 1) / ((long long)kBlock * ilp)); }
+
+// Every launch of a batched kernel: blocks of kBlock threads over n lanes, `ilp` lanes per thread; an empty batch launches
+// nothing, and b2s_launch_count() counts the rest.
+enum LaunchKind { kPlain, kPdl };
+template <LaunchKind K = kPlain, typename... KArgs, typename... Args>
+inline void launch(void (*kernel)(KArgs...), long long n, int ilp, cudaStream_t st, Args... args) {
+  if (n <= 0) return;
+  if constexpr (K == kPdl) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid_for(n, ilp));
+    cfg.blockDim = dim3(kBlock);
+    cfg.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  } else {
+    kernel<<<grid_for(n, ilp), kBlock, 0, st>>>(static_cast<KArgs>(args)...);
+  }
+  ++g_launches;
+}
+
+// ---- what the kernels do to one lane ---------------------------------------------------------------
+
+// State::ApplyAction on lane i (spiel.cc:441-451): a terminal lane or a rejected action is flagged and the lane stays as it
+// was; otherwise the new state is stored.  (a by reference: by value, nvcc 12.9 allocates k_apply<TicTacToeRules> differently.)
+template <class R>
+__device__ __forceinline__ void apply_or_flag(typename R::S& s, const int& a, const typename R::Cfg& cfg, const Ctx& ctx, long long i) {
+  if (R::terminal(s, cfg) || !R::apply(s, a, cfg, ctx, i)) { flag_error(ctx.err, ctx.lane0 + i); return; }
+  store_state<R>(s, cfg, ctx, i);
+}
+
+// Returns r of lane i into row i of rets[n][players].  kVec writes a two-player row as one 8-byte store and so needs rets
+// 8-byte aligned: the status and step kernels take it, b2s_rollout and b2s_record_trajectories do not promise that alignment.
+// (r is the caller's array: with it declared in here, nvcc 12.9 moves the state of k_rollout<LeducNRules> to local memory.)
+template <class R, bool kVec>
+__device__ __forceinline__ void store_returns(float* rets, long long i, const float* r, const typename R::Cfg& cfg) {
+  if (kVec && R::kPlayers == 2) reinterpret_cast<float2*>(rets)[i] = make_float2(r[0], r[1]);
+  else { const int np = rule_num_players<R>(cfg); for (int p = 0; p < np; ++p) rets[i * np + p] = r[p]; }
+}
+
+// The status byte of the compact env step (b2s_step_fused_host_compact), one per lane:
+//   bit 7      IsTerminal
+//   terminal:  bits 0-1 = outcome (0 draw / no winner, 1 player 0 won, 2 player 1 won) — win/loss/draw games only
+//   otherwise: bits 0-6 = LegalActionsMask when the game has <= 7 distinct actions (small_mask; connect_four <= 7 columns), else 0
+// m becomes the lane's next legal mask (zero when terminal) if small_mask or want_words asks for it.
+template <class R>
+__device__ __forceinline__ unsigned char status_byte(const typename R::S& s, const typename R::Cfg& cfg, int small_mask, bool want_words, u32* m) {
+  unsigned st = 0;
+  if (R::terminal(s, cfg)) {
+    float r[R::kPlayers];
+    R::returns(s, cfg, r);
+    st = 0x80u | (r[0] > 0.f ? 1u : (r[0] < 0.f ? 2u : 0u));
+    for (int w = 0; w < R::kMaskWords; ++w) m[w] = 0;
+  } else if (small_mask || want_words) {
+    R::legal_nonterminal(s, cfg, m);
+    if (small_mask) st = m[0] & 0x7Fu;
+  }
+  return (unsigned char)st;
 }
 
 // ---- kernels -------------------------------------------------------------------------------------
@@ -69,8 +119,7 @@ __global__ void __launch_bounds__(kBlock, R::kMinBlocks) k_apply(Ctx ctx, typena
     if (a[j] == -1) continue;
     typename R::S s;
     unpack_state<R>(s, pk[j], cfg);
-    if (R::terminal(s, cfg) || !R::apply(s, a[j], cfg, ctx, i)) { flag_error(ctx.err, ctx.lane0 + i); continue; }
-    store_state<R>(s, cfg, ctx, i);
+    apply_or_flag<R>(s, a[j], cfg, ctx, i);
   }
 }
 
@@ -108,6 +157,16 @@ __device__ __forceinline__ void store_masks_coalesced(u32* __restrict__ mask, lo
   __syncwarp();
 }
 
+// Row i of a legal-mask output mask[n][mask_words]: one-word masks are a plain store by live lanes, multi-word masks go through
+// store_masks_coalesced, so every thread of the warp must call it (live = false past n), uniformly over the grid.
+template <class R> using MaskStageFor = MaskStage<R::kMaskWords == 1 ? 0 : R::kMaskWords>;
+template <class R>
+__device__ __forceinline__ void store_mask_row(u32* __restrict__ mask, long long i, long long n, bool live, int mask_words, const u32* m,
+                                               MaskStageFor<R>& stage) {
+  if (R::kMaskWords == 1) { if (live) mask[i] = m[0]; }
+  else store_masks_coalesced(mask, i - (threadIdx.x & 31), n, live, mask_words, m, stage);
+}
+
 template <class R, int ILP>
 __global__ void __launch_bounds__(kBlock) k_legal_mask(Ctx ctx, typename R::Cfg cfg, u32* __restrict__ mask, int mask_words, long long n) {
   long long base = (long long)blockIdx.x * (kBlock * ILP) + threadIdx.x;
@@ -117,7 +176,7 @@ __global__ void __launch_bounds__(kBlock) k_legal_mask(Ctx ctx, typename R::Cfg 
     long long i = base + (long long)j * kBlock;
     if (i < n) fetch_state<R>(pk[j], ctx, i);
   }
-  __shared__ MaskStage<R::kMaskWords == 1 ? 0 : R::kMaskWords> stage;
+  __shared__ MaskStageFor<R> stage;
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
@@ -127,11 +186,7 @@ __global__ void __launch_bounds__(kBlock) k_legal_mask(Ctx ctx, typename R::Cfg 
       unpack_state<R>(s, pk[j], cfg);
       R::legal(s, cfg, m);
     }
-    if (R::kMaskWords == 1) {
-      if (i < n) mask[i] = m[0];
-    } else {
-      store_masks_coalesced(mask, i - (threadIdx.x & 31), n, i < n, mask_words, m, stage);
-    }
+    store_mask_row<R>(mask, i, n, i < n, mask_words, m, stage);
   }
 }
 
@@ -177,8 +232,7 @@ __global__ void __launch_bounds__(kBlock) k_status(Ctx ctx, typename R::Cfg cfg,
     if (rets) {
       float r[R::kPlayers];
       R::returns(s, cfg, r);
-      if (R::kPlayers == 2) reinterpret_cast<float2*>(rets)[i] = make_float2(r[0], r[1]);
-      else { const int np = rule_num_players<R>(cfg); for (int p = 0; p < np; ++p) rets[i * np + p] = r[p]; }
+      store_returns<R, true>(rets, i, r, cfg);
     }
   }
 }
@@ -197,7 +251,7 @@ __global__ void __launch_bounds__(kBlock) k_step_fused(Ctx ctx, typename R::Cfg 
     if (i < n) { a[j] = __ldg(actions + i); fetch_state<R>(pk[j], ctx, i); }
   }
   pdl_launch_dependents();
-  __shared__ MaskStage<R::kMaskWords == 1 ? 0 : R::kMaskWords> stage;
+  __shared__ MaskStageFor<R> stage;
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
@@ -206,37 +260,27 @@ __global__ void __launch_bounds__(kBlock) k_step_fused(Ctx ctx, typename R::Cfg 
     if (live) {
       typename R::S s;
       unpack_state<R>(s, pk[j], cfg);
-      if (a[j] != -1) {
-        if (R::terminal(s, cfg) || !R::apply(s, a[j], cfg, ctx, i)) flag_error(ctx.err, ctx.lane0 + i);
-        else store_state<R>(s, cfg, ctx, i);
-      }
+      if (a[j] != -1) apply_or_flag<R>(s, a[j], cfg, ctx, i);
       bool t = R::terminal(s, cfg);
       if (term) term[i] = t ? 1 : 0;
       if (rets) {
         float r[R::kPlayers];
         R::returns(s, cfg, r);
-        if (R::kPlayers == 2) reinterpret_cast<float2*>(rets)[i] = make_float2(r[0], r[1]);
-        else { const int np = rule_num_players<R>(cfg); for (int p = 0; p < np; ++p) rets[i * np + p] = r[p]; }
+        store_returns<R, true>(rets, i, r, cfg);
       }
       if (mask) {
         if (t) { for (int w = 0; w < R::kMaskWords; ++w) m[w] = 0; }
         else R::legal_nonterminal(s, cfg, m);
       }
     }
-    if (mask) {                                            // uniform over the grid
-      if (R::kMaskWords == 1) { if (live) mask[i] = m[0]; }
-      else store_masks_coalesced(mask, i - (threadIdx.x & 31), n, live, mask_words, m, stage);
-    }
+    if (mask) store_mask_row<R>(mask, i, n, live, mask_words, m, stage);
   }
 }
 
 // Compact env step for host-driven loops (b2s_step_fused_host_compact): the same apply -> terminal -> returns -> next legal
 // mask pass as k_step_fused with byte-wide I/O, because through PCIe the bytes per lane ARE the cost.  Actions are AT
-// (unsigned char: 0xFF = leave the lane untouched; int: -1).  One status byte per lane:
-//   bit 7      IsTerminal
-//   terminal:  bits 0-1 = outcome (0 draw / no winner, 1 player 0 won, 2 player 1 won) — win/loss/draw games only
-//   otherwise: bits 0-6 = LegalActionsMask when the game has <= 7 distinct actions (connect_four <= 7 columns), else 0
-// Games with more actions get their mask words through `mask` (nullable), exactly as k_step_fused writes them.
+// (unsigned char: 0xFF = leave the lane untouched; int: -1).  One status byte per lane (status_byte); games with more than 7
+// actions get their mask words through `mask` (nullable), exactly as k_step_fused writes them.
 template <class R, int ILP, class AT>
 __global__ void __launch_bounds__(kBlock) k_step_compact(Ctx ctx, typename R::Cfg cfg, const AT* __restrict__ actions, unsigned char* __restrict__ status,
                                                          u32* __restrict__ mask, int mask_words, int small_mask, long long n) {
@@ -255,7 +299,7 @@ __global__ void __launch_bounds__(kBlock) k_step_compact(Ctx ctx, typename R::Cf
     }
   }
   pdl_launch_dependents();
-  __shared__ MaskStage<R::kMaskWords == 1 ? 0 : R::kMaskWords> stage;
+  __shared__ MaskStageFor<R> stage;
 #pragma unroll
   for (int j = 0; j < ILP; ++j) {
     long long i = base + (long long)j * kBlock;
@@ -264,27 +308,10 @@ __global__ void __launch_bounds__(kBlock) k_step_compact(Ctx ctx, typename R::Cf
     if (live) {
       typename R::S s;
       unpack_state<R>(s, pk[j], cfg);
-      if (a[j] != -1) {
-        if (R::terminal(s, cfg) || !R::apply(s, a[j], cfg, ctx, i)) flag_error(ctx.err, ctx.lane0 + i);
-        else store_state<R>(s, cfg, ctx, i);
-      }
-      bool t = R::terminal(s, cfg);
-      unsigned st = 0;
-      if (t) {
-        float r[R::kPlayers];
-        R::returns(s, cfg, r);
-        st = 0x80u | (r[0] > 0.f ? 1u : (r[0] < 0.f ? 2u : 0u));
-        for (int w = 0; w < R::kMaskWords; ++w) m[w] = 0;
-      } else if (small_mask || mask) {
-        R::legal_nonterminal(s, cfg, m);
-        if (small_mask) st = m[0] & 0x7Fu;
-      }
-      status[i] = (unsigned char)st;
+      if (a[j] != -1) apply_or_flag<R>(s, a[j], cfg, ctx, i);
+      status[i] = status_byte<R>(s, cfg, small_mask, mask != nullptr, m);
     }
-    if (mask) {                                            // uniform over the grid
-      if (R::kMaskWords == 1) { if (live) mask[i] = m[0]; }
-      else store_masks_coalesced(mask, i - (threadIdx.x & 31), n, live, mask_words, m, stage);
-    }
+    if (mask) store_mask_row<R>(mask, i, n, live, mask_words, m, stage);
   }
 }
 
@@ -374,8 +401,7 @@ __global__ void __launch_bounds__(kBlock) k_rollout(Ctx ctx, typename R::Cfg cfg
   if (rets) {
     float r[R::kPlayers];
     R::returns(s, cfg, r);
-    const int np = rule_num_players<R>(cfg);
-    for (int p = 0; p < np; ++p) rets[i * np + p] = r[p];
+    store_returns<R, false>(rets, i, r, cfg);
   }
 }
 
@@ -386,18 +412,13 @@ __global__ void __launch_bounds__(kBlock) k_rollout(Ctx ctx, typename R::Cfg cfg
 //   decision of step t      k = philox_uniform(seed, g, 64 (t+1),         #legal)  -> k-th legal action (ascending)
 //   j-th chance node after   k = philox_uniform(seed, g, 64 (t+1) + 1 + j, #outcomes)   (before step 0: 64*0 + 1 + j)
 // (uniform policy = GetUniformPolicy; the chance distributions of kuhn / leduc are uniform over the listed outcomes).
-template <class R>
+template <class R, class Draw>
 __device__ __forceinline__ void traj_resolve_chance(typename R::S& s, const typename R::Cfg& cfg, const Ctx& ctx, long long i,
-                                                    u64 seed, u64 g, int mask_words, u32 b0) {
-  u32 j = 0;
-  while (R::cur_player(s, cfg) == kChancePlayerId) {
+                                                    int mask_words, Draw& draw, u32 b0) {
+  for (u32 j = 0; R::cur_player(s, cfg) == kChancePlayerId; ++j) {
     u32 m[R::kMaskWords];
     R::legal_nonterminal(s, cfg, m);
-    int cnt = 0;
-    for (int w = 0; w < mask_words; ++w) cnt += __popc(m[w]);
-    int a = nth_set_bit(m, mask_words, (int)philox_uniform(seed, g, b0 + 1u + j, (u32)cnt));
-    apply_known_legal<R>(s, a, cfg, ctx, i);
-    ++j;
+    apply_known_legal<R>(s, draw_legal(m, mask_words, draw, b0 + 1u + j), cfg, ctx, i);
   }
 }
 
@@ -409,7 +430,9 @@ __global__ void __launch_bounds__(kBlock) k_traj_begin(Ctx ctx, typename R::Cfg 
   typename R::S s;
   load_state<R>(s, cfg, ctx, i);
   if (R::cur_player(s, cfg) != kChancePlayerId) return;
-  traj_resolve_chance<R>(s, cfg, ctx, i, seed, (u64)(i + lane_offset), mask_words, 0u);
+  const u64 g = (u64)(i + lane_offset);
+  auto draw = [=](u32 b, u32 n) { return philox_uniform(seed, g, b, n); };
+  traj_resolve_chance<R>(s, cfg, ctx, i, mask_words, draw, 0u);
   store_state<R>(s, cfg, ctx, i);
 }
 
@@ -448,21 +471,9 @@ __global__ void __launch_bounds__(kBlock) k_step_compact_zc(Ctx ctx, typename R:
     typename R::S s;
     unpack_state<R>(s, pk[j], cfg);
     const unsigned raw = act_s[threadIdx.x + j * kBlock];
-    if (raw != 0xFFu) {
-      if (R::terminal(s, cfg) || !R::apply(s, (int)raw, cfg, ctx, i)) flag_error(ctx.err, ctx.lane0 + i);
-      else store_state<R>(s, cfg, ctx, i);
-    }
-    unsigned st = 0;
-    if (R::terminal(s, cfg)) {
-      float r[R::kPlayers];
-      R::returns(s, cfg, r);
-      st = 0x80u | (r[0] > 0.f ? 1u : (r[0] < 0.f ? 2u : 0u));
-    } else if (small_mask) {
-      u32 m[R::kMaskWords];
-      R::legal_nonterminal(s, cfg, m);
-      st = m[0] & 0x7Fu;
-    }
-    st_s[threadIdx.x + j * kBlock] = (unsigned char)st;
+    if (raw != 0xFFu) apply_or_flag<R>(s, (int)raw, cfg, ctx, i);
+    u32 m[R::kMaskWords];
+    st_s[threadIdx.x + j * kBlock] = status_byte<R>(s, cfg, small_mask, false, m);
   }
   __syncthreads();
   if (vec < here) {
@@ -484,7 +495,7 @@ template <class R>
 __global__ void __launch_bounds__(kBlock) k_traj_step(Ctx ctx, typename R::Cfg cfg, u64 seed, long long lane_offset, int t, int mask_words, int num_actions, TrajStepOut o, long long n) {
   long long i = (long long)blockIdx.x * kBlock + threadIdx.x;
   const bool live = i < n;
-  __shared__ MaskStage<R::kMaskWords == 1 ? 0 : R::kMaskWords> stage;
+  __shared__ MaskStageFor<R> stage;
   typename R::S s;
   u32 m[R::kMaskWords];
   int a = 0, pl = 0;
@@ -499,24 +510,20 @@ __global__ void __launch_bounds__(kBlock) k_traj_step(Ctx ctx, typename R::Cfg c
       }
     } else {
       const u64 g = (u64)(i + lane_offset);
+      auto draw = [=](u32 b, u32 n) { return philox_uniform(seed, g, b, n); };
       const u32 b0 = 64u * (u32)(t + 1);
       R::legal_nonterminal(s, cfg, m);
-      int cnt = 0;
-      for (int w = 0; w < mask_words; ++w) cnt += __popc(m[w]);
-      a = nth_set_bit(m, mask_words, (int)philox_uniform(seed, g, b0, (u32)cnt));
+      a = draw_legal(m, mask_words, draw, b0);
       pl = R::cur_player(s, cfg);
       valid = 1;
       apply_known_legal<R>(s, a, cfg, ctx, i);
-      traj_resolve_chance<R>(s, cfg, ctx, i, seed, g, mask_words, b0);
+      traj_resolve_chance<R>(s, cfg, ctx, i, mask_words, draw, b0);
       nit = R::terminal(s, cfg) ? 1 : 0;
       store_state<R>(s, cfg, ctx, i);
       if (nit && o.lengths) o.lengths[i] = t + 1;
     }
   }
-  if (o.mask) {                                            // uniform over the grid
-    if (R::kMaskWords == 1) { if (live) o.mask[i] = m[0]; }
-    else store_masks_coalesced(o.mask, i - (threadIdx.x & 31), n, live, mask_words, m, stage);
-  }
+  if (o.mask) store_mask_row<R>(o.mask, i, n, live, mask_words, m, stage);
   if (!live) return;
   if (o.actions) o.actions[i] = a;
   if (o.players) o.players[i] = (signed char)pl;
@@ -536,31 +543,25 @@ __global__ void __launch_bounds__(kBlock) k_traj_finish(Ctx ctx, typename R::Cfg
   if (rewards) {
     float r[R::kPlayers];
     R::returns(s, cfg, r);
-    const int np = rule_num_players<R>(cfg);
-    for (int p = 0; p < np; ++p) rewards[i * np + p] = r[p];
+    store_returns<R, false>(rewards, i, r, cfg);
   }
 }
 
-// Clone: copy lane `src` of one batch into lanes [dst0, dst0+count) of another.
+// Clone: lane sl of one batch into lane dl of another, with its history.
 template <class R>
-__global__ void __launch_bounds__(kBlock) k_broadcast(Ctx dst, long long dst0, long long count, Ctx srcctx, long long src, typename R::Cfg cfg) {
-  long long i = (long long)blockIdx.x * kBlock + threadIdx.x;
-  if (i >= count) return;
+__device__ __forceinline__ void clone_lane(const Ctx& dst, long long dl, const Ctx& srcctx, long long sl, const typename R::Cfg& cfg) {
   typename R::S s;
-  load_state<R>(s, cfg, srcctx, src);
-  store_state<R>(s, cfg, dst, dst0 + i);
-  R::copy_history(dst, dst0 + i, srcctx, src, s, cfg);
+  load_state<R>(s, cfg, srcctx, sl);
+  store_state<R>(s, cfg, dst, dl);
+  R::copy_history(dst, dl, srcctx, sl, s, cfg);
 }
 
-// Clone a lane range: dst[dst0 + i] = src[src0 + i].
+// Clone a lane range: dst[dst0 + i] = src[src0 + i * src_step]; src_step 1 copies a range, 0 copies lane src0 into every lane.
 template <class R>
-__global__ void __launch_bounds__(kBlock) k_copy(Ctx dst, long long dst0, Ctx srcctx, long long src0, long long count, typename R::Cfg cfg) {
+__global__ void __launch_bounds__(kBlock) k_copy(Ctx dst, long long dst0, Ctx srcctx, long long src0, int src_step, long long count, typename R::Cfg cfg) {
   long long i = (long long)blockIdx.x * kBlock + threadIdx.x;
   if (i >= count) return;
-  typename R::S s;
-  load_state<R>(s, cfg, srcctx, src0 + i);
-  store_state<R>(s, cfg, dst, dst0 + i);
-  R::copy_history(dst, dst0 + i, srcctx, src0 + i, s, cfg);
+  clone_lane<R>(dst, dst0 + i, srcctx, src0 + i * src_step, cfg);
 }
 
 // Clone lanes [0, count) into the lane-blob form (R::store, as b2s_state_get returns a lane): the MCTS kernel reads its roots
@@ -582,10 +583,7 @@ __global__ void __launch_bounds__(kBlock) k_gather(Ctx dst, Ctx srcctx, const lo
   if (i >= count) return;
   long long sl = src_lanes[i];
   if (sl < 0 || sl >= srcctx.cap) { flag_error(dst.err, i); return; }
-  typename R::S s;
-  load_state<R>(s, cfg, srcctx, sl);
-  store_state<R>(s, cfg, dst, i);
-  R::copy_history(dst, i, srcctx, sl, s, cfg);
+  clone_lane<R>(dst, i, srcctx, sl, cfg);
 }
 
 // ---- host-side per-game dispatch table --------------------------------------------------------------
@@ -616,8 +614,8 @@ struct GameOps {
   // uint8 actions and status bytes in device-mapped HOST memory, no mask words (k_step_compact_zc)
   virtual void step_compact_zero_copy(const Ctx&, const unsigned char* a_host, unsigned char* status_host, long long n, cudaStream_t) = 0;
   virtual void rollout(const Ctx&, u64 seed, long long lane_offset, float* rets, int* plies, long long n, cudaStream_t) = 0;
-  virtual void broadcast(const Ctx& dst, long long dst0, long long count, const Ctx& src, long long srclane, cudaStream_t) = 0;
-  virtual void copy(const Ctx& dst, long long dst0, const Ctx& src, long long src0, long long count, cudaStream_t) = 0;
+  // dst[dst0 + i] = src[src0 + i * src_step], src_step 0 (one lane into all) or 1
+  virtual void copy(const Ctx& dst, long long dst0, const Ctx& src, long long src0, int src_step, long long count, cudaStream_t) = 0;
   virtual void copy_to_blob(const Ctx& dst, const Ctx& src, long long count, cudaStream_t) = 0;   // dst in the lane-blob form
   virtual void gather(const Ctx& dst, const Ctx& src, const long long* src_lanes, long long count, cudaStream_t) = 0;
   virtual void traj_begin(const Ctx&, u64 seed, long long lane_offset, int* lengths, long long n, cudaStream_t) = 0;
@@ -632,30 +630,6 @@ struct GameOps {
   virtual void mcts_eval_report(long long n, const struct MctsEvalArgs& args, cudaStream_t) = 0;
   b2s_game_info info;
 };
-
-// A lane's blob is its stored chunks, or for a rule core with R::Packed the decoded state written by R::store.
-template <class R, class Q = typename R::Packed>
-void stored_to_blob_impl(const typename R::Cfg& c, const void* stored, void* blob, int) {
-  typename R::S s;
-  R::unpack(s, *static_cast<const Q*>(stored), c);
-  Ctx b = {};
-  b.planes = blob; b.cap = 1;
-  R::store(s, b, 0);
-}
-template <class R>
-void stored_to_blob_impl(const typename R::Cfg&, const void* stored, void* blob, long) { memcpy(blob, stored, sizeof(typename R::Chunk) * R::kChunks); }
-template <class R, class Q = typename R::Packed>
-void blob_to_stored_impl(const typename R::Cfg& c, const void* blob, void* stored, int) {
-  typename R::S s;
-  Ctx b = {};
-  b.planes = const_cast<void*>(blob); b.cap = 1;
-  R::load(s, b, 0);
-  *static_cast<Q*>(stored) = R::pack(s, c);
-}
-template <class R>
-void blob_to_stored_impl(const typename R::Cfg&, const void* blob, void* stored, long) { memcpy(stored, blob, sizeof(typename R::Chunk) * R::kChunks); }
-
-inline unsigned grid_for(long long n, int ilp = 1) { return (unsigned)((n + (long long)kBlock * ilp - 1) / ((long long)kBlock * ilp)); }
 
 // magic M with floor(e*M >> 32) == e / d for all 0 <= e < limit (checked exhaustively).
 inline bool make_magic(int d, int limit, u32* out) {
@@ -683,28 +657,44 @@ struct GameOpsT : GameOps {
   }
   void device_init() override { call_device_init<R>(0); }
   size_t chunk_bytes() const override { return sizeof(StoredChunk<R>); }
-  void stored_to_blob(const void* stored, void* blob) const override { stored_to_blob_impl<R>(cfg, stored, blob, 0); }
-  void blob_to_stored(const void* blob, void* stored) const override { blob_to_stored_impl<R>(cfg, blob, stored, 0); }
+  // A lane's blob is its stored chunks, or for a rule core with R::Packed the decoded state written by R::store.
+  void stored_to_blob(const void* stored, void* blob) const override {
+    if constexpr (has_packed<R>::value) {
+      typename R::S s;
+      R::unpack(s, *static_cast<const typename R::Packed*>(stored), cfg);
+      Ctx b = {};
+      b.planes = blob; b.cap = 1;
+      R::store(s, b, 0);
+    } else {
+      memcpy(blob, stored, sizeof(typename R::Chunk) * R::kChunks);
+    }
+  }
+  void blob_to_stored(const void* blob, void* stored) const override {
+    if constexpr (has_packed<R>::value) {
+      typename R::S s;
+      Ctx b = {};
+      b.planes = const_cast<void*>(blob); b.cap = 1;
+      R::load(s, b, 0);
+      *static_cast<typename R::Packed*>(stored) = R::pack(s, cfg);
+    } else {
+      memcpy(stored, blob, sizeof(typename R::Chunk) * R::kChunks);
+    }
+  }
   int chunks() const override { return R::kChunks; }
   void reset(const Ctx& c, long long n, cudaStream_t st) override {
-    long long m = n > 0 ? n : 1;
-    k_reset<R><<<grid_for(m), kBlock, 0, st>>>(c, cfg, n); ++g_launches;
+    launch(k_reset<R>, n > 0 ? n : 1, 1, st, c, cfg, n);     // at least one block: lane 0 clears the error record
   }
   void apply(const Ctx& c, const int* a, long long n, cudaStream_t st) override {
-    if (n <= 0) return;
-    launch_pdl(k_apply<R, R::kIlp>, grid_for(n, R::kIlp), st, c, cfg, a, n); ++g_launches;
+    launch<kPdl>(k_apply<R, R::kIlp>, n, R::kIlp, st, c, cfg, a, n);
   }
   void legal_mask(const Ctx& c, u32* m, long long n, cudaStream_t st) override {
-    if (n <= 0) return;
-    k_legal_mask<R, R::kIlp><<<grid_for(n, R::kIlp), kBlock, 0, st>>>(c, cfg, m, info.mask_words, n); ++g_launches;
+    launch(k_legal_mask<R, R::kIlp>, n, R::kIlp, st, c, cfg, m, info.mask_words, n);
   }
   void legal_list(const Ctx& c, short* out, int* counts, int stride, long long n, cudaStream_t st) override {
-    if (n <= 0) return;
-    k_legal_list<R><<<grid_for(n), kBlock, 0, st>>>(c, cfg, out, counts, stride, info.mask_words, n); ++g_launches;
+    launch(k_legal_list<R>, n, 1, st, c, cfg, out, counts, stride, info.mask_words, n);
   }
   void status(const Ctx& c, signed char* cur, unsigned char* term, float* rets, long long n, cudaStream_t st) override {
-    if (n <= 0) return;
-    k_status<R, R::kIlp><<<grid_for(n, R::kIlp), kBlock, 0, st>>>(c, cfg, cur, term, rets, n); ++g_launches;
+    launch(k_status<R, R::kIlp>, n, R::kIlp, st, c, cfg, cur, term, rets, n);
   }
   const char* obs(const Ctx& c, int player, int which, int zero_terminal, float* out, long long n, cudaStream_t st) override {
     int size = which == 0 ? info.observation_tensor_size : info.information_state_tensor_size;
@@ -713,63 +703,47 @@ struct GameOpsT : GameOps {
     if (n <= 0) return nullptr;
     u32 magic;
     if (!make_magic(size, 32 * size, &magic)) return "internal: no division magic";
-    k_obs<R><<<grid_for(n), kBlock, 0, st>>>(c, cfg, player, which, zero_terminal, out, size, magic, n); ++g_launches;
+    launch(k_obs<R>, n, 1, st, c, cfg, player, which, zero_terminal, out, size, magic, n);
     return nullptr;
   }
   void step_fused(const Ctx& c, const int* a, u32* m, unsigned char* term, float* rets, long long n, cudaStream_t st) override {
-    if (n <= 0) return;
-    launch_pdl(k_step_fused<R, R::kIlp>, grid_for(n, R::kIlp), st, c, cfg, a, m, info.mask_words, term, rets, n); ++g_launches;
+    launch<kPdl>(k_step_fused<R, R::kIlp>, n, R::kIlp, st, c, cfg, a, m, info.mask_words, term, rets, n);
   }
+  int small_mask() const { return info.num_distinct_actions <= 7 ? 1 : 0; }   // the legal mask fits the status byte
   void step_compact(const Ctx& c, const void* a, int action_bytes, unsigned char* status, u32* m, long long n, cudaStream_t st) override {
-    if (n <= 0) return;
-    const int small_mask = info.num_distinct_actions <= 7 ? 1 : 0;
     if (action_bytes == 1)
-      launch_pdl(k_step_compact<R, R::kIlp, unsigned char>, grid_for(n, R::kIlp), st, c, cfg, (const unsigned char*)a, status, m, info.mask_words, small_mask, n);
+      launch<kPdl>(k_step_compact<R, R::kIlp, unsigned char>, n, R::kIlp, st, c, cfg, (const unsigned char*)a, status, m, info.mask_words, small_mask(), n);
     else
-      launch_pdl(k_step_compact<R, R::kIlp, int>, grid_for(n, R::kIlp), st, c, cfg, (const int*)a, status, m, info.mask_words, small_mask, n);
-    ++g_launches;
+      launch<kPdl>(k_step_compact<R, R::kIlp, int>, n, R::kIlp, st, c, cfg, (const int*)a, status, m, info.mask_words, small_mask(), n);
   }
   void step_compact_zero_copy(const Ctx& c, const unsigned char* a_host, unsigned char* status_host, long long n, cudaStream_t st) override {
-    if (n <= 0) return;
-    const int small_mask = info.num_distinct_actions <= 7 ? 1 : 0;
-    k_step_compact_zc<R, R::kIlp><<<grid_for(n, R::kIlp), kBlock, 0, st>>>(c, cfg, a_host, status_host, small_mask, n); ++g_launches;
+    launch(k_step_compact_zc<R, R::kIlp>, n, R::kIlp, st, c, cfg, a_host, status_host, small_mask(), n);
   }
   void rollout(const Ctx& c, u64 seed, long long lane_offset, float* rets, int* plies, long long n, cudaStream_t st) override {
-    if (n <= 0) return;
-    k_rollout<R><<<grid_for(n), kBlock, 0, st>>>(c, cfg, seed, lane_offset, info.mask_words, info.max_game_length + 4, rets, plies, n); ++g_launches;
+    launch(k_rollout<R>, n, 1, st, c, cfg, seed, lane_offset, info.mask_words, info.max_game_length + 4, rets, plies, n);
   }
-  void broadcast(const Ctx& dst, long long dst0, long long count, const Ctx& src, long long srclane, cudaStream_t st) override {
-    if (count <= 0) return;
-    k_broadcast<R><<<grid_for(count), kBlock, 0, st>>>(dst, dst0, count, src, srclane, cfg); ++g_launches;
+  void copy(const Ctx& dst, long long dst0, const Ctx& src, long long src0, int src_step, long long count, cudaStream_t st) override {
+    launch(k_copy<R>, count, 1, st, dst, dst0, src, src0, src_step, count, cfg);
+  }
+  void copy_to_blob(const Ctx& dst, const Ctx& src, long long count, cudaStream_t st) override {
+    launch(k_copy_to_blob<R>, count, 1, st, dst, src, count, cfg);
+  }
+  void gather(const Ctx& dst, const Ctx& src, const long long* src_lanes, long long count, cudaStream_t st) override {
+    launch(k_gather<R>, count, 1, st, dst, src, src_lanes, count, cfg);
   }
   void traj_begin(const Ctx& c, u64 seed, long long lane_offset, int* lengths, long long n, cudaStream_t st) override {
-    if (n <= 0) return;
-    k_traj_begin<R><<<grid_for(n), kBlock, 0, st>>>(c, cfg, seed, lane_offset, info.mask_words, lengths, n); ++g_launches;
+    launch(k_traj_begin<R>, n, 1, st, c, cfg, seed, lane_offset, info.mask_words, lengths, n);
   }
   void traj_step(const Ctx& c, u64 seed, long long lane_offset, int t, const TrajStepOut& o, long long n, cudaStream_t st) override {
-    if (n <= 0) return;
-    k_traj_step<R><<<grid_for(n), kBlock, 0, st>>>(c, cfg, seed, lane_offset, t, info.mask_words, info.num_distinct_actions, o, n); ++g_launches;
+    launch(k_traj_step<R>, n, 1, st, c, cfg, seed, lane_offset, t, info.mask_words, info.num_distinct_actions, o, n);
   }
   void traj_finish(const Ctx& c, float* rewards, long long n, cudaStream_t st) override {
-    if (n <= 0) return;
-    k_traj_finish<R><<<grid_for(n), kBlock, 0, st>>>(c, cfg, rewards, n); ++g_launches;
+    launch(k_traj_finish<R>, n, 1, st, c, cfg, rewards, n);
   }
   const char* mcts(const Ctx& roots, const Ctx& work, long long n, const MctsArgs& args, cudaStream_t st) override;
   const char* mcts_eval_limits(int* max_legal, int* max_path) const override;
   void mcts_eval_step(const Ctx& roots, const Ctx& leaves, long long n, const MctsEvalArgs& args, cudaStream_t st) override;
   void mcts_eval_report(long long n, const MctsEvalArgs& args, cudaStream_t st) override;
-  void gather(const Ctx& dst, const Ctx& src, const long long* src_lanes, long long count, cudaStream_t st) override {
-    if (count <= 0) return;
-    k_gather<R><<<grid_for(count), kBlock, 0, st>>>(dst, src, src_lanes, count, cfg); ++g_launches;
-  }
-  void copy_to_blob(const Ctx& dst, const Ctx& src, long long count, cudaStream_t st) override {
-    if (count <= 0) return;
-    k_copy_to_blob<R><<<grid_for(count), kBlock, 0, st>>>(dst, src, count, cfg); ++g_launches;
-  }
-  void copy(const Ctx& dst, long long dst0, const Ctx& src, long long src0, long long count, cudaStream_t st) override {
-    if (count <= 0) return;
-    k_copy<R><<<grid_for(count), kBlock, 0, st>>>(dst, dst0, src, src0, count, cfg); ++g_launches;
-  }
 };
 
 }  // namespace b2s

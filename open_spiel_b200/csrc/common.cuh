@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/b2s.h"
 
 namespace b2s {
@@ -84,6 +86,15 @@ __device__ __forceinline__ int nth_set_bit(const u32* words, int nwords, int k) 
   return -1;
 }
 
+// A uniformly random legal action of the mask: the draw(b, n)-th set bit, n = the number of set bits.  `draw(b, n)` returns a
+// uniform integer in [0, n) from random block b.
+template <class Draw>
+__device__ __forceinline__ int draw_legal(const u32* m, int mask_words, Draw& draw, u32 b) {
+  int cnt = 0;
+  for (int w = 0; w < mask_words; ++w) cnt += __popc(m[w]);
+  return nth_set_bit(m, mask_words, (int)draw(b, (u32)cnt));
+}
+
 // R::apply_legal(...) when the rule core offers a cheaper "already known legal" path, else R::apply(...)
 template <class R, class S, class Cfg>
 __device__ __forceinline__ auto apply_known_legal_impl(S& s, int a, const Cfg& c, const Ctx& ctx, long long lane, int)
@@ -111,40 +122,32 @@ __device__ __forceinline__ int rule_num_players(const Cfg& c) { return rule_num_
 // holds one R::Packed per lane in a single plane, R::pack(s, cfg) encodes it and R::unpack(s, p, cfg) decodes it
 // (connect_four: the column height is in the configuration).  The streaming kernels fetch all their lanes before they
 // unpack any, so every load of a thread is in flight at once; Fetched<R> is what they hold in between.
-template <class R> auto fetched_of(int) -> typename R::Packed;
-template <class R> auto fetched_of(long) -> typename R::S;
-template <class R> using Fetched = decltype(fetched_of<R>(0));
-template <class R> auto stored_of(int) -> typename R::Packed;
-template <class R> auto stored_of(long) -> typename R::Chunk;
-template <class R> using StoredChunk = decltype(stored_of<R>(0));   // one chunk of a lane as a batch holds it
-template <class R, class P, class Q = typename R::Packed>
-__device__ __forceinline__ void fetch_state_impl(P& p, const Ctx& ctx, long long i, int) { p = reinterpret_cast<const Q*>(ctx.planes)[i]; }
-template <class R, class P>
-__device__ __forceinline__ void fetch_state_impl(P& p, const Ctx& ctx, long long i, long) { R::load(p, ctx, i); }
-template <class R, class P>
-__device__ __forceinline__ void fetch_state(P& p, const Ctx& ctx, long long i) { fetch_state_impl<R>(p, ctx, i, 0); }
-template <class R, class S, class P, class Cfg, class Q = typename R::Packed>
-__device__ __forceinline__ void unpack_state_impl(S& s, const P& p, const Cfg& c, int) { R::unpack(s, p, c); }
-template <class R, class S, class P, class Cfg>
-__device__ __forceinline__ void unpack_state_impl(S& s, const P& p, const Cfg&, long) { s = p; }
-template <class R, class S, class P, class Cfg>
-__device__ __forceinline__ void unpack_state(S& s, const P& p, const Cfg& c) { unpack_state_impl<R>(s, p, c, 0); }
-template <class R, class S, class Cfg, class Q = typename R::Packed>
-__device__ __forceinline__ void load_state_impl(S& s, const Cfg& c, const Ctx& ctx, long long i, int) {
-  R::unpack(s, reinterpret_cast<const Q*>(ctx.planes)[i], c);
+template <class R, class = void> struct has_packed : std::false_type {};
+template <class R> struct has_packed<R, std::void_t<typename R::Packed>> : std::true_type {};
+template <class R, bool = has_packed<R>::value> struct LaneLayout { typedef typename R::S Fetched; typedef typename R::Chunk Stored; };
+template <class R> struct LaneLayout<R, true> { typedef typename R::Packed Fetched; typedef typename R::Packed Stored; };
+template <class R> using Fetched = typename LaneLayout<R>::Fetched;
+template <class R> using StoredChunk = typename LaneLayout<R>::Stored;   // one chunk of a lane as a batch holds it
+template <class R>
+__device__ __forceinline__ void fetch_state(Fetched<R>& p, const Ctx& ctx, long long i) {
+  if constexpr (has_packed<R>::value) p = reinterpret_cast<const typename R::Packed*>(ctx.planes)[i];
+  else R::load(p, ctx, i);
 }
-template <class R, class S, class Cfg>
-__device__ __forceinline__ void load_state_impl(S& s, const Cfg&, const Ctx& ctx, long long i, long) { R::load(s, ctx, i); }
-template <class R, class S, class Cfg>
-__device__ __forceinline__ void load_state(S& s, const Cfg& c, const Ctx& ctx, long long i) { load_state_impl<R>(s, c, ctx, i, 0); }
-template <class R, class S, class Cfg, class Q = typename R::Packed>
-__device__ __forceinline__ void store_state_impl(const S& s, const Cfg& c, const Ctx& ctx, long long i, int) {
-  reinterpret_cast<Q*>(ctx.planes)[i] = R::pack(s, c);
+template <class R>
+__device__ __forceinline__ void unpack_state(typename R::S& s, const Fetched<R>& p, const typename R::Cfg& c) {
+  if constexpr (has_packed<R>::value) R::unpack(s, p, c);
+  else s = p;
 }
-template <class R, class S, class Cfg>
-__device__ __forceinline__ void store_state_impl(const S& s, const Cfg&, const Ctx& ctx, long long i, long) { R::store(s, ctx, i); }
-template <class R, class S, class Cfg>
-__device__ __forceinline__ void store_state(const S& s, const Cfg& c, const Ctx& ctx, long long i) { store_state_impl<R>(s, c, ctx, i, 0); }
+template <class R>
+__device__ __forceinline__ void load_state(typename R::S& s, const typename R::Cfg& c, const Ctx& ctx, long long i) {
+  if constexpr (has_packed<R>::value) R::unpack(s, reinterpret_cast<const typename R::Packed*>(ctx.planes)[i], c);
+  else R::load(s, ctx, i);
+}
+template <class R>
+__device__ __forceinline__ void store_state(const typename R::S& s, const typename R::Cfg& c, const Ctx& ctx, long long i) {
+  if constexpr (has_packed<R>::value) reinterpret_cast<typename R::Packed*>(ctx.planes)[i] = R::pack(s, c);
+  else R::store(s, ctx, i);
+}
 
 // One playout step: choose a uniformly random legal action and apply it; returns the action.
 // Rule cores may expose a cheap candidate superset (R::num_candidates / R::candidate, e.g. go: empty non-ko points
@@ -165,9 +168,7 @@ __device__ __forceinline__ int playout_step_impl(S& s, const Cfg& c, const Ctx& 
                                                  Draw& draw, u32 ply, long) {
   u32 m[R::kMaskWords];
   R::legal_nonterminal(s, c, m);
-  int cnt = 0;
-  for (int w = 0; w < mask_words; ++w) cnt += __popc(m[w]);
-  int a = nth_set_bit(m, mask_words, (int)draw(ply, (u32)cnt));
+  int a = draw_legal(m, mask_words, draw, ply);
   apply_known_legal<R>(s, a, c, ctx, lane);
   return a;
 }
