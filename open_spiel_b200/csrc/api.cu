@@ -617,6 +617,45 @@ int b2s_gather_states(void* dst_batch, void* src_batch, const int64_t* src_lanes
 }
 
 // ---- MCTS ---------------------------------------------------------------------------------------------------
+// log_table[k] = std::log((double)k) for k < need, filled by the host so UCT values equal the CPU's; `*have` is the size of the
+// table already at *table (0 = none), which is kept when it is large enough
+static int mcts_log_table(double** table, int* have, int need, cudaStream_t st) {
+  if (*have >= need) return 0;
+  if (*table) cudaFree(*table);
+  *table = nullptr; *have = 0;
+  std::vector<double> t(need);
+  for (int k = 0; k < need; ++k) t[k] = std::log((double)k);
+  CU(cudaMalloc((void**)table, sizeof(double) * need));
+  CU(cudaMemcpyAsync(*table, t.data(), sizeof(double) * need, cudaMemcpyHostToDevice, st));
+  *have = need;
+  return 0;
+}
+
+// Nodes per tree arena.  With max_nodes_total: its share.  Otherwise the worst case of `factor` blocks of at most A nodes per
+// simulation, capped by 60 % of the free device memory plus `reusable_bytes` (an arena about to be replaced) and, with a node
+// budget, by `factor` times twice the budget: the budget is logical (MCTSBot::nodes_, live nodes <= budget + one expansion),
+// and blocks freed by the collector are reused by exact size (a pruned node re-expands to the same number of children) or
+// split, never coalesced.  A tree that still cannot allocate stops and is reported by b2s_error_count.  0: too small for one
+// expansion of every tree.
+static unsigned long long mcts_nodes_per_tree(long long max_nodes_total, int max_simulations, long long max_nodes_per_tree,
+                                              long long n_trees, unsigned long long A, size_t node_bytes, size_t free_bytes,
+                                              unsigned long long reusable_bytes, unsigned long long factor) {
+  unsigned long long per_tree;
+  if (max_nodes_total > 0) {
+    per_tree = (unsigned long long)max_nodes_total / (unsigned long long)n_trees;
+  } else {
+    const unsigned long long worst = 2ull + factor * (unsigned long long)max_simulations * A;
+    const unsigned long long fit = (unsigned long long)((free_bytes + reusable_bytes) * 0.6 / node_bytes) / (unsigned long long)n_trees;
+    per_tree = worst < fit ? worst : fit;
+    if (max_nodes_per_tree > 1) {
+      const unsigned long long want = factor * (2ull * (unsigned long long)max_nodes_per_tree + 8 * A + 64);
+      if (want < per_tree) per_tree = want;
+    }
+  }
+  if (per_tree > 0xffffffffull) per_tree = 0xffffffffull;
+  return per_tree < factor * A + 2 ? 0 : per_tree;
+}
+
 int b2s_mcts_search(void* roots_batch, int64_t n_trees, const b2s_mcts_config* cfg, int32_t* visit_counts_d,
                     double* total_reward_d, float* outcome_p0_d, int32_t* best_action_d, int32_t* sims_run_d,
                     void* stream) {
@@ -642,41 +681,18 @@ int b2s_mcts_search(void* roots_batch, int64_t n_trees, const b2s_mcts_config* c
   Ctx work;
   work.planes = B->mcts_work; work.cap = B->mcts_work_cap; work.hist = B->mcts_hist; work.err = B->err;
   B->ops->copy_to_blob(work, B->ctx(), n_trees, st);
-  // log table filled by the host's std::log
-  int need = cfg->max_simulations + 2;
-  if (B->mcts_log_n < need) {
-    if (B->mcts_log) cudaFree(B->mcts_log);
-    B->mcts_log = nullptr; B->mcts_log_n = 0;
-    std::vector<double> t(need);
-    for (int k = 0; k < need; ++k) t[k] = std::log((double)k);
-    CU(cudaMalloc((void**)&B->mcts_log, sizeof(double) * need));
-    CU(cudaMemcpy(B->mcts_log, t.data(), sizeof(double) * need, cudaMemcpyHostToDevice));
-    B->mcts_log_n = need;
-  }
+  if (int r = mcts_log_table(&B->mcts_log, &B->mcts_log_n, cfg->max_simulations + 2, st)) return r;
   // node arenas, one per tree (mcts.cuh): nodes_per_tree slots of 16 B (n_rollouts a power of two) or 24 B
   const unsigned long long A = (unsigned long long)B->info.num_distinct_actions;
   const long long work_units = (long long)cfg->max_simulations * cfg->n_rollouts;
   const int compact = (cfg->n_rollouts & (cfg->n_rollouts - 1)) == 0 && work_units < (1ll << 30);
   const size_t node_bytes = compact ? sizeof(MctsNodeC) : sizeof(MctsNodeW);
-  unsigned long long per_tree;
-  if (cfg->max_nodes_total > 0) {
-    per_tree = (unsigned long long)cfg->max_nodes_total / (unsigned long long)n_trees;
-  } else {
-    const unsigned long long worst = 2ull + (unsigned long long)cfg->max_simulations * A;      // one expansion per simulation at most
-    size_t free_b = 0, total_b = 0;
-    CU(cudaMemGetInfo(&free_b, &total_b));
-    const unsigned long long fit = (unsigned long long)((free_b + B->mcts_pool_bytes) * 0.6 / node_bytes) / (unsigned long long)n_trees;
-    per_tree = worst < fit ? worst : fit;
-    if (cfg->max_nodes_per_tree > 1) {
-      // the budget is logical (MCTSBot::nodes_, live nodes <= budget + one expansion); blocks freed by the collector are reused
-      // by exact size (a pruned node re-expands to the same number of children) or split, never coalesced, so the arena is
-      // twice the budget; a tree that still cannot allocate stops and is reported by b2s_error_count
-      const unsigned long long want = 2ull * (unsigned long long)cfg->max_nodes_per_tree + 8 * A + 64;
-      if (want < per_tree) per_tree = want;
-    }
-  }
-  if (per_tree > 0xffffffffull) per_tree = 0xffffffffull;
-  if (per_tree < A + 2) return fail("mcts: node arena too small (max_nodes_total / free memory)");
+  size_t free_b = 0, total_b = 0;
+  if (cfg->max_nodes_total <= 0) CU(cudaMemGetInfo(&free_b, &total_b));
+  // one expansion per simulation at most
+  const unsigned long long per_tree = mcts_nodes_per_tree(cfg->max_nodes_total, cfg->max_simulations, cfg->max_nodes_per_tree, n_trees,
+                                                          A, node_bytes, free_b, B->mcts_pool_bytes, 1);
+  if (!per_tree) return fail("mcts: node arena too small (max_nodes_total / free memory)");
   if (cfg->max_nodes_per_tree > 0x7fffffffll) return fail("mcts: max_nodes_per_tree out of range");
   const unsigned long long want_bytes = per_tree * (unsigned long long)n_trees * node_bytes;
   if (B->mcts_pool_bytes < want_bytes) {
@@ -761,22 +777,11 @@ int b2s_mcts_eval_create(void* roots_batch, int64_t n_trees, const b2s_mcts_eval
   const size_t N = (size_t)n_trees, A = (size_t)B->info.num_distinct_actions;
   // arena: every simulation allocates at most one block for an expansion and one for a prior cache; caches stop at half of it
   const size_t node_bytes = sizeof(MctsNodeE);
-  unsigned long long per_tree;
-  if (cfg->max_nodes_total > 0) {
-    per_tree = (unsigned long long)cfg->max_nodes_total / (unsigned long long)n_trees;
-  } else {
-    const unsigned long long worst = 2ull + 2ull * (unsigned long long)cfg->max_simulations * A;
-    size_t free_b = 0, total_b = 0;
-    CU(cudaMemGetInfo(&free_b, &total_b));
-    const unsigned long long fit = (unsigned long long)(free_b * 0.6 / node_bytes) / (unsigned long long)n_trees;
-    per_tree = worst < fit ? worst : fit;
-    if (cfg->max_nodes_per_tree > 1) {   // as b2s_mcts_search's budgeted arena (twice the budget), twice over for the caches
-      const unsigned long long want = 4ull * (unsigned long long)cfg->max_nodes_per_tree + 16 * A + 128;
-      if (want < per_tree) per_tree = want;
-    }
-  }
-  if (per_tree > 0xffffffffull) per_tree = 0xffffffffull;
-  if (per_tree < 2 * A + 2) return fail("mcts_eval: node arena too small (max_nodes_total / free memory)");
+  size_t free_b = 0, total_b = 0;
+  if (cfg->max_nodes_total <= 0) CU(cudaMemGetInfo(&free_b, &total_b));
+  const unsigned long long per_tree = mcts_nodes_per_tree(cfg->max_nodes_total, cfg->max_simulations, cfg->max_nodes_per_tree, n_trees,
+                                                          A, node_bytes, free_b, 0, 2);
+  if (!per_tree) return fail("mcts_eval: node arena too small (max_nodes_total / free memory)");
   CU(cudaMalloc(&S->roots, (size_t)B->info.state_bytes * (size_t)L->cap));
   CU(cudaMalloc((void**)&S->pool, per_tree * N * node_bytes));
   CU(cudaMalloc((void**)&S->trees, sizeof(MctsEvalTree) * N));
@@ -784,13 +789,8 @@ int b2s_mcts_eval_create(void* roots_batch, int64_t n_trees, const b2s_mcts_eval
   CU(cudaMalloc((void**)&S->path, sizeof(u32) * (size_t)max_path * N));
   CU(cudaMalloc((void**)&S->pending, N));
   CU(cudaMalloc((void**)&S->n_pending, sizeof(unsigned long long)));
-  {
-    const int need = cfg->max_simulations + 2;
-    std::vector<double> t(need);
-    for (int k = 0; k < need; ++k) t[k] = std::log((double)k);
-    CU(cudaMalloc((void**)&S->log_table, sizeof(double) * need));
-    CU(cudaMemcpyAsync(S->log_table, t.data(), sizeof(double) * need, cudaMemcpyHostToDevice, st));
-  }
+  int log_n = 0;
+  if (int r = mcts_log_table(&S->log_table, &log_n, cfg->max_simulations + 2, st)) return r;
   if (cfg->root_noise_d) {         // the search keeps its own copy: the caller may reuse the buffer
     CU(cudaMalloc((void**)&S->noise, sizeof(double) * A * N));
     CU(cudaMemcpyAsync(S->noise, cfg->root_noise_d, sizeof(double) * A * N, cudaMemcpyDeviceToDevice, st));
