@@ -213,6 +213,59 @@ typedef struct b2s_trajectory_out {
 int b2s_record_trajectories(void* batch, uint64_t seed, int64_t lane_offset, int64_t n, int32_t max_unroll_length,
                             const b2s_trajectory_out* out, void* stream);
 
+/* ---- RL environment ------------------------------------------------------------------------ */
+
+/* open_spiel/python/rl_environment.py Environment over every lane of a batch, stepped as
+ * vector_env.py SyncVectorEnv.step: one call is one time step of lanes [0, n), enqueued on `stream`, with no
+ * host synchronisation, so it can be captured in a CUDA graph.  Per lane, with a = actions_d[i]:
+ *   lane terminal (the previous call returned LAST): Environment.step after LAST (rl_environment.py:372-373):
+ *                   a is ignored; the lane restarts from the initial state, chance resolved; FIRST, rewards 0, done 0.
+ *   a == -1:        the lane is untouched; MID (it is not terminal, see above).
+ *   otherwise:      ApplyAction(a), then chance nodes are sampled until a decision node or a terminal state
+ *                   (_sample_external_events, :431-442); rewards = State::Rewards() (0 until terminal, then Returns()),
+ *                   done = terminal, LAST if terminal else MID.  An illegal action leaves the lane as it was (MID,
+ *                   rewards 0) and is counted by b2s_error_count.
+ *   reset_if_done and done: as SyncVectorEnv.step(reset_if_done=True) (vector_env.py:54-64): rewards and done stay
+ *                   those of the step; the lane restarts (chance resolved) and the observation, legal mask, current
+ *                   player and step type written are the new episode's FIRST time step.  The terminal observations
+ *                   (unreset_time_steps) are not kept.
+ * b2s_env_reset is Environment.reset of lanes [0, n): initial state, chance resolved, FIRST, rewards 0.  Unlike
+ * b2s_reset it leaves the error counter alone.  Lanes must come from b2s_env_reset or b2s_env_step: the batch's own
+ * initial state is a chance node in kuhn_poker / leduc_poker, which Environment never exposes.
+ * Outputs (device pointers, each may be NULL):
+ *   observations   [P][n][F] float32, player-major: row p is InformationStateTensor(p) or ObservationTensor(p)
+ *   legal_mask     [n][mask_words] uint32, the player to move's LegalActionsMask as bits; all zero at LAST
+ *   rewards        [n][P] float32;  done [n] uint8;  step_type [n] uint8 (FIRST 0, MID 1, LAST 2);
+ *   current_player [n] int8 (-4 at terminal)
+ * Discounts are not written: they are discount * (step_type != LAST).
+ * Random stream: the call with counter c (0 for the env's first call) takes chance node j after the action from
+ * Philox block 64 (c + 1) + 1 + j and chance node j after a reset from block 64 (c + 1) + 32 + j, keyed by
+ * (seed, lane + lane_offset): the k-th outcome of the chance node's legal mask, k uniform in [0, #outcomes)
+ * (csrc/common.cuh philox_uniform).  c lives in device memory and advances by one per b2s_env_step / b2s_env_reset
+ * in stream order, so replays of a captured call draw fresh outcomes; its period is 2^26 calls.  Results do not depend
+ * on how lanes are split over batches or GPUs (a shard of lanes [k, k + m) uses lane_offset k).
+ * observation: 0 ObservationTensor, 1 InformationStateTensor (kuhn_poker, leduc_poker), -1 the information state
+ * when the game has one, else the observation (rl_environment.py:228-241).  The env refers to the batch, which must
+ * outlive it. */
+typedef struct b2s_env_config {
+  uint64_t seed;
+  int64_t  lane_offset;
+  int32_t  observation;
+  int32_t  reserved;     /* 0 */
+} b2s_env_config;
+typedef struct b2s_env_out {
+  float*    observations;
+  uint32_t* legal_mask;
+  float*    rewards;
+  uint8_t*  done;
+  uint8_t*  step_type;
+  int8_t*   current_player;
+} b2s_env_out;
+int  b2s_env_create(void* batch, const b2s_env_config* cfg, void** out_env);
+int  b2s_env_reset(void* env, int64_t n, const b2s_env_out* out, void* stream);
+int  b2s_env_step(void* env, const int32_t* actions_d, int reset_if_done, int64_t n, const b2s_env_out* out, void* stream);
+void b2s_env_destroy(void* env);
+
 /* ---- MCTS ---------------------------------------------------------------------------------- */
 
 /* Replaces algorithms::MCTSBot (open_spiel/algorithms/mcts.h:149-230) with a RandomRolloutEvaluator

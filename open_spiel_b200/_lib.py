@@ -57,6 +57,15 @@ class TrajectoryOut(C.Structure):
                 ("rewards", C.c_void_p), ("lengths", C.c_void_p)]
 
 
+class EnvConfig(C.Structure):
+    _fields_ = [("seed", C.c_uint64), ("lane_offset", C.c_int64), ("observation", C.c_int32), ("reserved", C.c_int32)]
+
+
+class EnvOut(C.Structure):
+    _fields_ = [("observations", C.c_void_p), ("legal_mask", C.c_void_p), ("rewards", C.c_void_p), ("done", C.c_void_p),
+                ("step_type", C.c_void_p), ("current_player", C.c_void_p)]
+
+
 class CfrInfo(C.Structure):
     _fields_ = [("num_nodes", C.c_int32), ("num_levels", C.c_int32), ("num_infosets", C.c_int32),
                 ("num_entries", C.c_int32), ("key_floats", C.c_int32), ("iteration", C.c_int32),
@@ -95,6 +104,10 @@ SIGNATURES = {
     "b2s_mcts_search": (C.c_int, [_VP, _I64, C.POINTER(MctsConfig), _VP, _VP, _VP, _VP, _VP, _VP]),
     "b2s_mcts_nodes_used": (C.c_int, [_VP, C.POINTER(_I64)]),
     "b2s_gather_states": (C.c_int, [_VP, _VP, _VP, _I64, _VP]),
+    "b2s_env_create": (C.c_int, [_VP, C.POINTER(EnvConfig), C.POINTER(_VP)]),
+    "b2s_env_reset": (C.c_int, [_VP, _I64, C.POINTER(EnvOut), _VP]),
+    "b2s_env_step": (C.c_int, [_VP, _VP, C.c_int, _I64, C.POINTER(EnvOut), _VP]),
+    "b2s_env_destroy": (None, [_VP]),
     "b2s_mcts_eval_create": (C.c_int, [_VP, _I64, C.POINTER(MctsEvalConfig), _VP, C.POINTER(_VP), _VP]),
     "b2s_mcts_eval_step": (C.c_int, [_VP, _VP, _VP, _VP, C.POINTER(_I64), _VP]),
     "b2s_mcts_eval_results": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),

@@ -605,6 +605,84 @@ int b2s_record_trajectories(void* batch, uint64_t seed, int64_t lane_offset, int
   return post();
 }
 
+}  // extern "C"
+
+// ---- RL environment (k_env_step) -------------------------------------------------------------------------------------
+namespace b2s {
+struct Env {
+  Batch* batch = nullptr;
+  b2s_env_config cfg;
+  int which = 0;                            // 0 ObservationTensor, 1 InformationStateTensor
+  unsigned long long* counter = nullptr;    // calls so far (device memory): the random block of the next call
+  ~Env() {
+    if (counter) { cudaSetDevice(batch->device); cudaFree(counter); }
+  }
+};
+
+__global__ void k_env_tick(unsigned long long* counter) { *counter += 1; }
+
+// One call: the lane step (actions == nullptr: reset), every player's tensor row, then the counter.
+static int env_call(Env* E, const int32_t* actions_d, int reset_if_done, int64_t n, const b2s_env_out* out, void* stream) {
+  if (int r = check(E->batch, n)) return r;
+  if (!out) return fail("env: null output descriptor");
+  if (out->observations && ((uintptr_t)out->observations & 3u)) return fail("env: observations must be 4-byte aligned");
+  Batch* B = E->batch;
+  cudaStream_t st = (cudaStream_t)stream;
+  EnvStepOut o;
+  o.mask = out->legal_mask; o.rewards = out->rewards; o.done = out->done; o.step_type = out->step_type; o.cur = out->current_player;
+  B->ops->env_step(B->ctx(), actions_d, reset_if_done, E->cfg.seed, E->cfg.lane_offset, E->counter, o, n, st);
+  if (out->observations) {
+    const size_t F = (size_t)(E->which ? B->info.information_state_tensor_size : B->info.observation_tensor_size);
+    for (int p = 0; p < B->info.num_players; ++p)
+      if (const char* e = B->ops->obs(B->ctx(), p, E->which, 0, out->observations + (size_t)p * (size_t)n * F, n, st)) return fail(e);
+  }
+  k_env_tick<<<1, 1, 0, st>>>(E->counter);
+  ++g_launches;
+  return post();
+}
+}  // namespace b2s
+
+extern "C" {
+
+int b2s_env_create(void* batch, const b2s_env_config* cfg, void** out_env) {
+  if (!out_env) return fail("env: null out_env");
+  *out_env = nullptr;
+  if (int r = check(batch, 0)) return r;
+  if (!cfg) return fail("env: null config");
+  if (cfg->reserved != 0) return fail("env: reserved must be 0");
+  Batch* B = (Batch*)batch;
+  const bool has_info = B->info.information_state_tensor_size > 0, has_obs = B->info.observation_tensor_size > 0;
+  int which;
+  switch (cfg->observation) {
+    case -1: which = has_info ? 1 : 0; break;
+    case 0: which = 0; break;
+    case 1: which = 1; break;
+    default: return fail("env: observation must be -1, 0 or 1");
+  }
+  if (which == 1 && !has_info) return fail("env: the game provides no information state tensor");
+  if (which == 0 && !has_obs) return fail("env: the game provides no observation tensor");
+  std::unique_ptr<Env> E(new Env);
+  E->batch = B; E->cfg = *cfg; E->which = which;
+  CU(cudaMalloc((void**)&E->counter, sizeof(unsigned long long)));
+  CU(cudaMemset(E->counter, 0, sizeof(unsigned long long)));
+  CU(cudaDeviceSynchronize());              // the first call may come on any stream
+  *out_env = E.release();
+  return 0;
+}
+
+int b2s_env_reset(void* env, int64_t n, const b2s_env_out* out, void* stream) {
+  if (!env) return fail("env: null env");
+  return env_call((Env*)env, nullptr, 0, n, out, stream);
+}
+
+int b2s_env_step(void* env, const int32_t* actions_d, int reset_if_done, int64_t n, const b2s_env_out* out, void* stream) {
+  if (!env) return fail("env: null env");
+  if (!actions_d) return fail("env: null actions");
+  return env_call((Env*)env, actions_d, reset_if_done, n, out, stream);
+}
+
+void b2s_env_destroy(void* env) { delete (Env*)env; }
+
 int b2s_gather_states(void* dst_batch, void* src_batch, const int64_t* src_lanes_d, int64_t count, void* stream) {
   if (int r = check(dst_batch, count)) return r;
   if (!src_batch || !src_lanes_d) return fail("gather: null argument");

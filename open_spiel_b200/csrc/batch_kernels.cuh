@@ -6,6 +6,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "env_step.cuh"
 
 namespace b2s {
 
@@ -412,15 +413,6 @@ __global__ void __launch_bounds__(kBlock) k_rollout(Ctx ctx, typename R::Cfg cfg
 //   decision of step t      k = philox_uniform(seed, g, 64 (t+1),         #legal)  -> k-th legal action (ascending)
 //   j-th chance node after   k = philox_uniform(seed, g, 64 (t+1) + 1 + j, #outcomes)   (before step 0: 64*0 + 1 + j)
 // (uniform policy = GetUniformPolicy; the chance distributions of kuhn / leduc are uniform over the listed outcomes).
-template <class R, class Draw>
-__device__ __forceinline__ void traj_resolve_chance(typename R::S& s, const typename R::Cfg& cfg, const Ctx& ctx, long long i,
-                                                    int mask_words, Draw& draw, u32 b0) {
-  for (u32 j = 0; R::cur_player(s, cfg) == kChancePlayerId; ++j) {
-    u32 m[R::kMaskWords];
-    R::legal_nonterminal(s, cfg, m);
-    apply_known_legal<R>(s, draw_legal(m, mask_words, draw, b0 + 1u + j), cfg, ctx, i);
-  }
-}
 
 template <class R>
 __global__ void __launch_bounds__(kBlock) k_traj_begin(Ctx ctx, typename R::Cfg cfg, u64 seed, long long lane_offset, int mask_words, int* __restrict__ lengths, long long n) {
@@ -479,6 +471,61 @@ __global__ void __launch_bounds__(kBlock) k_step_compact_zc(Ctx ctx, typename R:
   if (vec < here) {
     if (vec + 16 <= here) *reinterpret_cast<uint4*>(status + b0 + vec) = *reinterpret_cast<const uint4*>(st_s + vec);
     else for (int k = vec; k < here; ++k) status[b0 + k] = st_s[k];
+  }
+}
+
+// ---- RL environment step (b2s_env_step / b2s_env_reset; per-lane body env_step_lane, env_step.cuh) ---------------------
+struct EnvStepOut {           // any pointer may be null
+  u32* mask;                  // [n][mask_words] of the player to move, zero at LAST
+  float* rewards;             // [n][num_players]
+  unsigned char* done;        // [n]
+  unsigned char* step_type;   // [n] EnvStepType
+  signed char* cur;           // [n] current player
+};
+
+// actions == nullptr: Environment.reset of every lane.  The call's random blocks come from *counter (device memory, advanced
+// by a later launch of the same call), so a replayed CUDA graph of the call draws fresh chance outcomes.
+template <class R, int ILP>
+__global__ void __launch_bounds__(kBlock) k_env_step(Ctx ctx, typename R::Cfg cfg, const int* __restrict__ actions, int reset_if_done,
+                                                     u64 seed, long long lane_offset, const unsigned long long* __restrict__ counter,
+                                                     int mask_words, EnvStepOut o, long long n) {
+  long long base = (long long)blockIdx.x * (kBlock * ILP) + threadIdx.x;
+  int a[ILP];
+  Fetched<R> pk[ILP];
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) {
+    long long i = base + (long long)j * kBlock;
+    a[j] = -1;
+    if (i < n && actions) { a[j] = __ldg(actions + i); fetch_state<R>(pk[j], ctx, i); }
+  }
+  const u32 b0 = env_block(*counter);
+  __shared__ MaskStageFor<R> stage;
+#pragma unroll
+  for (int j = 0; j < ILP; ++j) {
+    long long i = base + (long long)j * kBlock;
+    const bool live = i < n;
+    u32 m[R::kMaskWords];
+    if (live) {
+      typename R::S s;
+      if (actions) unpack_state<R>(s, pk[j], cfg);
+      const u64 g = (u64)(i + lane_offset);
+      auto draw = [=](u32 b, u32 k) { return philox_uniform(seed, g, b, k); };
+      float r[R::kPlayers];
+      unsigned char done;
+      bool changed;
+      const unsigned char st = env_step_lane<R>(s, a[j], actions == nullptr, reset_if_done != 0, cfg, ctx, i, mask_words, draw, b0, r, done, changed);
+      if (changed) store_state<R>(s, cfg, ctx, i);
+      const int cp = R::cur_player(s, cfg);
+      if (o.rewards) store_returns<R, false>(o.rewards, i, r, cfg);
+      if (o.done) o.done[i] = done;
+      if (o.step_type) o.step_type[i] = st;
+      if (o.cur) o.cur[i] = (signed char)cp;
+      if (o.mask) {
+        if (cp == kTerminalPlayerId) { for (int w = 0; w < R::kMaskWords; ++w) m[w] = 0; }
+        else R::legal_nonterminal(s, cfg, m);
+      }
+    }
+    if (o.mask) store_mask_row<R>(o.mask, i, n, live, mask_words, m, stage);
   }
 }
 
@@ -621,6 +668,9 @@ struct GameOps {
   virtual void traj_begin(const Ctx&, u64 seed, long long lane_offset, int* lengths, long long n, cudaStream_t) = 0;
   virtual void traj_step(const Ctx&, u64 seed, long long lane_offset, int t, const TrajStepOut& o, long long n, cudaStream_t) = 0;
   virtual void traj_finish(const Ctx&, float* rewards, long long n, cudaStream_t) = 0;
+  // RL environment step of lanes [0, n) (k_env_step); actions == nullptr resets every lane
+  virtual void env_step(const Ctx&, const int* a, int reset_if_done, u64 seed, long long lane_offset, const unsigned long long* counter,
+                        const EnvStepOut& o, long long n, cudaStream_t) = 0;
   // MCTS over n roots (mcts.cuh); returns an error string when the game has no device MCTS
   virtual const char* mcts(const Ctx& roots, const Ctx& work, long long n, const struct MctsArgs& args, cudaStream_t) = 0;
   // caller-evaluated MCTS (mcts_eval.cuh): the children-block and path-stack sizes of the game's device search, or an error
@@ -739,6 +789,10 @@ struct GameOpsT : GameOps {
   }
   void traj_finish(const Ctx& c, float* rewards, long long n, cudaStream_t st) override {
     launch(k_traj_finish<R>, n, 1, st, c, cfg, rewards, n);
+  }
+  void env_step(const Ctx& c, const int* a, int reset_if_done, u64 seed, long long lane_offset, const unsigned long long* counter,
+                const EnvStepOut& o, long long n, cudaStream_t st) override {
+    launch(k_env_step<R, R::kIlp>, n, R::kIlp, st, c, cfg, a, reset_if_done, seed, lane_offset, counter, info.mask_words, o, n);
   }
   const char* mcts(const Ctx& roots, const Ctx& work, long long n, const MctsArgs& args, cudaStream_t st) override;
   const char* mcts_eval_limits(int* max_legal, int* max_path) const override;

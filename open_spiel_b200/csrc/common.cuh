@@ -177,6 +177,18 @@ __device__ __forceinline__ int playout_step(S& s, const Cfg& c, const Ctx& ctx, 
   return playout_step_impl<R>(s, c, ctx, lane, mask_words, draw, ply, 0);
 }
 
+// Apply chance outcomes until the state is a decision node or terminal: the j-th chance node takes the draw(b0 + 1 + j, #outcomes)-th
+// outcome of its legal mask (the trajectory recorder and the RL environment step key their chance draws so).
+template <class R, class Draw>
+__device__ __forceinline__ void traj_resolve_chance(typename R::S& s, const typename R::Cfg& cfg, const Ctx& ctx, long long i,
+                                                    int mask_words, Draw& draw, u32 b0) {
+  for (u32 j = 0; R::cur_player(s, cfg) == kChancePlayerId; ++j) {
+    u32 m[R::kMaskWords];
+    R::legal_nonterminal(s, cfg, m);
+    apply_known_legal<R>(s, draw_legal(m, mask_words, draw, b0 + 1u + j), cfg, ctx, i);
+  }
+}
+
 // ---- 128-bit bitboards (hex: up to 121 cells; go: 9 rows x 10-bit stride) ------------------------------------
 struct B128 {
   u64 lo, hi;

@@ -478,6 +478,115 @@ class BatchedTrajectory:
         return la / la.sum(-1, keepdim=True).clamp_(min=1) * self.valid.unsqueeze(-1) + la * (1 - self.valid.unsqueeze(-1))
 
 
+class StepType:
+    """rl_environment.StepType values as step_type holds them."""
+    FIRST = 0
+    MID = 1
+    LAST = 2
+
+
+class ObservationType:
+    """rl_environment.ObservationType (rl_environment.py:78-81); VectorEnv also takes the reference's enum members."""
+    INFORMATION_STATE = 0
+    OBSERVATION = 1
+
+
+class VectorTimeStep:
+    """The time steps of all envs (rl_environment.TimeStep of each lane, stacked): info_state [n, P, F] float32,
+    legal_actions_mask [n, A] bool (the player to move's; all False at LAST), current_player [n] int8, rewards [n, P]
+    float32 (0 at FIRST where the reference has None), discounts [n, P] float32 (0 at LAST, `discount` otherwise, also at
+    FIRST where the reference has None), step_type [n] uint8 (StepType).  Views of the env's buffers, which the next
+    reset() / step() overwrites."""
+
+    def __init__(self, info_state, legal_actions_mask, current_player, rewards, discounts, step_type):
+        self.info_state, self.legal_actions_mask, self.current_player = info_state, legal_actions_mask, current_player
+        self.rewards, self.discounts, self.step_type = rewards, discounts, step_type
+
+    def first(self):
+        return self.step_type == StepType.FIRST
+
+    def last(self):
+        return self.step_type == StepType.LAST
+
+
+class VectorEnv:
+    """rl_environment.Environment over `num_envs` lanes, stepped as vector_env.SyncVectorEnv (b2s_env_*): one reset() or
+    step() is a fixed set of kernel launches on the current torch stream with no host synchronisation, so `policy
+    forward + env.step` can be captured into a torch.cuda.CUDAGraph.  Chance nodes are sampled on the device from a
+    Philox stream keyed by (seed, lane + lane_offset, call number) instead of the reference's numpy ChanceEventSampler.
+    observation_type None = information state when the game has one, else observation (rl_environment.py:228-241).
+    env.batch is the underlying BatchedState."""
+
+    def __init__(self, game, num_envs, seed=0, observation_type=None, discount=1.0, lane_offset=0, device=0):
+        from ._lib import EnvConfig, EnvOut
+        if isinstance(game, str):
+            game = load_game(game)
+        self.game, self.num_envs, self.discount = game, int(num_envs), float(discount)
+        self.batch = BatchedState(game, self.num_envs, device)
+        info, dev, n = self.batch.info, self.batch._dev, self.num_envs
+        kind = getattr(observation_type, "name", observation_type)
+        which = {None: -1, ObservationType.OBSERVATION: 0, "OBSERVATION": 0,
+                 ObservationType.INFORMATION_STATE: 1, "INFORMATION_STATE": 1}.get(kind)
+        if which is None:
+            raise B2SError("VectorEnv: unknown observation_type %r" % (observation_type,))
+        self._h = C.c_void_p()
+        check(lib().b2s_env_create(self.batch._h, C.byref(EnvConfig(int(seed), int(lane_offset), which, 0)), C.byref(self._h)))
+        if which == -1:
+            which = 1 if info.information_state_tensor_size > 0 else 0
+        F = info.information_state_tensor_size if which == 1 else info.observation_tensor_size
+        P, A = info.num_players, info.num_distinct_actions
+        self._obs = torch.empty((P, n, F), dtype=torch.float32, device=dev)     # player-major, as the kernels write it
+        self._mask_words = torch.empty((n, info.mask_words), dtype=torch.int32, device=dev)
+        self._rewards = torch.empty((n, P), dtype=torch.float32, device=dev)
+        self._done = torch.empty((n,), dtype=torch.uint8, device=dev)
+        self._step_type = torch.empty((n,), dtype=torch.uint8, device=dev)
+        self._cur = torch.empty((n,), dtype=torch.int8, device=dev)
+        self._mask = torch.empty((n, A), dtype=torch.bool, device=dev)
+        self._discounts = torch.empty((n, P), dtype=torch.float32, device=dev)
+        self._bits = torch.arange(32, dtype=torch.int32, device=dev)
+        self._out = EnvOut(self._obs.data_ptr(), self._mask_words.data_ptr(), self._rewards.data_ptr(), self._done.data_ptr(),
+                           self._step_type.data_ptr(), self._cur.data_ptr())
+        self._started = False
+        self.time_step = VectorTimeStep(self._obs.permute(1, 0, 2), self._mask, self._cur, self._rewards, self._discounts,
+                                        self._step_type)
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib().b2s_env_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def _finish(self):
+        n, A = self.num_envs, self._mask.shape[1]
+        bits = (self._mask_words.unsqueeze(-1) >> self._bits) & 1
+        self._mask.copy_(bits.reshape(n, -1)[:, :A])
+        torch.mul((self._step_type != StepType.LAST).unsqueeze(1).expand_as(self._discounts), self.discount, out=self._discounts)
+        return self.time_step
+
+    def reset(self):
+        """SyncVectorEnv.reset(): Environment.reset of every env.  Returns the VectorTimeStep (all FIRST)."""
+        check(lib().b2s_env_reset(self._h, self.num_envs, C.byref(self._out), self.batch._stream()))
+        self._started = True
+        return self._finish()
+
+    def step(self, actions, reset_if_done=False):
+        """SyncVectorEnv.step(actions, reset_if_done): returns (time_step, reward [n, P], done [n] bool), the first three
+        results of the reference (unreset_time_steps is not kept).  actions [n] is an integer CUDA tensor, -1 leaves an
+        env untouched; envs at LAST ignore their action and start a new episode.  An env never reset is reset, as
+        Environment.step does before its first reset()."""
+        if not self._started:
+            return self.reset(), self._rewards, self._done.view(torch.bool)
+        if actions.dtype != torch.int32 or not actions.is_contiguous():
+            actions = actions.to(torch.int32).contiguous()
+        if not actions.is_cuda or actions.numel() != self.num_envs:
+            raise B2SError("VectorEnv.step: actions must be a CUDA tensor of %d integers" % self.num_envs)
+        check(lib().b2s_env_step(self._h, actions.data_ptr(), int(bool(reset_if_done)), self.num_envs, C.byref(self._out),
+                                 self.batch._stream()))
+        return self._finish(), self._rewards, self._done.view(torch.bool)
+
+
 class ChildSelectionPolicy:
     """algorithms::ChildSelectionPolicy (mcts.h:148)."""
     UCT = 0
