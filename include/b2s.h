@@ -353,6 +353,45 @@ int  b2s_mcts_eval_results(void* search, int32_t* visit_counts_d, double* total_
                            void* stream);
 void b2s_mcts_eval_destroy(void* search);
 
+/* ---- AlphaBetaSearch -------------------------------------------------------------------------- */
+
+/* algorithms::AlphaBetaSearch(game, state, value_function = {}, depth_limit, maximizing_player) (open_spiel/algorithms/
+ * minimax.cc:49-137, 221-258) from each of lanes [0, n) of roots_batch, run entirely on the device, one result per lane:
+ *   - legal actions are searched in ascending order; a MAX node keeps the first child whose value is strictly greater, a MIN
+ *     node the first whose value is strictly smaller; alpha = max(alpha, value) / beta = min(beta, value), and the remaining
+ *     children are cut when alpha >= beta.  The root starts at (-inf, +inf), so it keeps scanning after it finds a win.
+ *   - depth_limit < 0 is unlimited (the reference's counter never reaches 0); maximizing_player -1 (kInvalidPlayer) is the
+ *     root's current player.  No value function, no move ordering, no transposition table: node counts and tied best actions
+ *     are the reference's.
+ * Outputs (device, nullable), lane i:
+ *   value_d        double: PlayerReturn(maximizing_player) of the solved root (-1, 0 or +1 for every served game).
+ *   best_action_d  int32: the reference's best_action; -1 (kInvalidAction) for a terminal root.
+ *   nodes_d        int64: child states generated below the root (the reference's ApplyAction / Child calls).
+ *   status_d       uint8: 0 solved;
+ *                  1 the budget ran out: the lane stopped before generating child number max_nodes_per_root + 1 (value NaN,
+ *                    best action -1; a device addition: a lane is solved iff the reference generates <= max_nodes_per_root);
+ *                  2 a non-terminal state at depth 0 (the reference's SpielFatalError: there is no value function);
+ *                  3 maximizing_player -1 on a terminal root (the reference indexes the returns with player -4).
+ *                  Statuses 2 and 3 leave value NaN and best action -1 and are counted by b2s_error_count on roots_batch
+ *                  (status 1 is not: the caller asked for the budget).
+ * Games: tic_tac_toe, connect_four, breakthrough, hex, go 2..9, mnk, othello, y and havannah, every configuration the batch
+ * accepts.  kuhn_poker and leduc_poker (AlphaBetaSearch checks kDeterministic) and go 10..19 return an error.
+ * Each thread searches one root at a time and takes the next root from a device counter when it is done.  Its stack of
+ * (max_game_length + 2) frames (the state, its unsearched legal actions, alpha, beta, value) lives in a buffer the batch
+ * allocates on its first call; the grid is sized so that buffer stays within B2S_ALPHA_BETA_STACK_BYTES, and games whose
+ * deepest stack exceeds B2S_ALPHA_BETA_THREAD_STACK_BYTES per thread are not served (go 10..19).  Enqueued on `stream`, no
+ * synchronisation; calls on one batch must be ordered on the device (they share the stack and the counter).  An unbudgeted
+ * search of an early position of a large game runs for as long as the reference's would take on one core per root. */
+#define B2S_ALPHA_BETA_STACK_BYTES (1ull << 30)
+#define B2S_ALPHA_BETA_THREAD_STACK_BYTES (64u << 10)
+typedef struct b2s_alpha_beta_config {
+  int32_t depth_limit;          /* < 0: unlimited */
+  int32_t maximizing_player;    /* -1 (the root's current player), 0 or 1 */
+  int64_t max_nodes_per_root;   /* 0 = unlimited */
+} b2s_alpha_beta_config;
+int b2s_alpha_beta_search(void* roots_batch, int64_t n, const b2s_alpha_beta_config* cfg, double* value_d,
+                          int32_t* best_action_d, int64_t* nodes_d, uint8_t* status_d, void* stream);
+
 /* ---- CFR ----------------------------------------------------------------------------------- */
 
 /* Replaces algorithms::CFRSolver / CFRPlusSolver (open_spiel/algorithms/cfr.h:312-357) for two-player

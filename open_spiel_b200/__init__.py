@@ -7,4 +7,4 @@ C ABI in include/b2s.h (libb2s.so); torch is used only for device buffers and st
 """
 from ._lib import B2SError as SpielError  # noqa: F401
 from .spiel import (BatchedState, BatchedTrajectory, CFRSolver, ChildSelectionPolicy, ExternalSamplingMCCFRSolver, OutcomeSamplingMCCFRSolver, Game, ObservationType, StepType, VectorEnv, VectorTimeStep, MCTSBot, MCTSEvalSearch, RandomRolloutEvaluator, State, load_game, bind_host_to_device, mcts_nodes_used,
-                    dirichlet_noise, mcts_search, mcts_search_evaluated, registered_names)  # noqa: F401
+                    alpha_beta_search, dirichlet_noise, mcts_search, mcts_search_evaluated, registered_names)  # noqa: F401

@@ -51,6 +51,10 @@ class MctsEvalConfig(C.Structure):
                 ("root_noise_d", C.c_void_p)]
 
 
+class AlphaBetaConfig(C.Structure):
+    _fields_ = [("depth_limit", C.c_int32), ("maximizing_player", C.c_int32), ("max_nodes_per_root", C.c_int64)]
+
+
 class TrajectoryOut(C.Structure):
     _fields_ = [("observations", C.c_void_p), ("legal_mask", C.c_void_p), ("actions", C.c_void_p),
                 ("player_ids", C.c_void_p), ("valid", C.c_void_p), ("next_is_terminal", C.c_void_p),
@@ -112,6 +116,7 @@ SIGNATURES = {
     "b2s_mcts_eval_step": (C.c_int, [_VP, _VP, _VP, _VP, C.POINTER(_I64), _VP]),
     "b2s_mcts_eval_results": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "b2s_mcts_eval_destroy": (None, [_VP]),
+    "b2s_alpha_beta_search": (C.c_int, [_VP, _I64, C.POINTER(AlphaBetaConfig), _VP, _VP, _VP, _VP, _VP]),
     "b2s_cfr_create": (C.c_int, [C.c_int, C.POINTER(Params), C.c_int, C.c_int, C.POINTER(_VP)]),
     "b2s_cfr_destroy": (None, [_VP]),
     "b2s_cfr_iterate": (C.c_int, [_VP, C.c_int, _VP]),

@@ -39,6 +39,54 @@ int GameIdAndParams(const Game& game, b2s_params* p) {
   return gid;
 }
 
+// ---- AlphaBetaSearch -------------------------------------------------------------------------------------------
+std::pair<double, Action> AlphaBetaSearch(const Game& game, const State* state, std::function<double(const State&)> value_function,
+                                          int depth_limit, Player maximizing_player, bool use_undo) {
+  const int gid = value_function ? -1 : b2s_game_id(game.GetType().short_name.c_str());
+  std::shared_ptr<const Game> packed_game = gid >= 0 ? B200Game::Create(game.GetType(), game.GetParameters()) : nullptr;
+  // kInvalidPlayer (the root's mover) is the C ABI's -1
+  b2s_alpha_beta_config cfg = {depth_limit, maximizing_player == kInvalidPlayer ? -1 : maximizing_player, 0};
+  void* batch = nullptr;
+  if (packed_game && (maximizing_player == kInvalidPlayer || maximizing_player == 0 || maximizing_player == 1)) {
+    // the packed game's own parameters (it reads every game's, e.g. mnk's m, n, k)
+    const B200Game& pg = static_cast<const B200Game&>(*packed_game);
+    Check(b2s_batch_create(gid, &pg.cparams(), 1, 0, &batch));
+    // a search of no roots checks only the game: kuhn_poker, leduc_poker and go 10..19 are not served on the device
+    if (b2s_alpha_beta_search(batch, 0, &cfg, nullptr, nullptr, nullptr, nullptr, nullptr) != 0) {
+      b2s_batch_destroy(batch);
+      batch = nullptr;
+    }
+  }
+  if (!batch) return algorithms::AlphaBetaSearch(game, state, value_function, depth_limit, maximizing_player, use_undo);
+  // the root as a packed lane, rebuilt from its history when it is not a B200State (as B200MCTSBot::RootToDevice)
+  std::unique_ptr<State> root = packed_game->NewInitialState();
+  const B200State* packed = state ? dynamic_cast<const B200State*>(state) : nullptr;
+  if (!packed) {
+    if (state)
+      for (Action a : state->History()) root->ApplyAction(a);
+    packed = static_cast<const B200State*>(root.get());
+  }
+  packed->ToBatchLane(batch, 0);
+  void* dev = nullptr;
+  Check(b2s_device_alloc(0, &dev, 32));
+  char* d = (char*)dev;
+  Check(b2s_alpha_beta_search(batch, 1, &cfg, (double*)d, (int32_t*)(d + 16), (int64_t*)(d + 8), (uint8_t*)(d + 20), nullptr));
+  char out[32];
+  Check(b2s_memcpy_d2h(0, out, dev, sizeof out, nullptr));
+  Check(b2s_stream_synchronize(0, nullptr));
+  b2s_device_free(0, dev);
+  b2s_batch_destroy(batch);
+  double value;
+  int32_t best;
+  memcpy(&value, out, sizeof value);
+  memcpy(&best, out + 16, sizeof best);
+  switch ((uint8_t)out[20]) {
+    case 2: SpielFatalError("We assume we can walk the full depth of the tree. Try increasing depth or provide a value_function.");
+    case 3: SpielFatalError("AlphaBetaSearch: maximizing_player is kInvalidPlayer at a terminal state");
+  }
+  return {value, (Action)best};
+}
+
 // ---- MCTS ------------------------------------------------------------------------------------------------------
 B200MCTSBot::B200MCTSBot(const Game& game, int n_rollouts, double uct_c, int max_simulations, int64_t max_memory_mb,
                          bool solve, int seed, bool verbose, algorithms::ChildSelectionPolicy policy) {

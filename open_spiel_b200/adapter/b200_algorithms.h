@@ -14,6 +14,7 @@
 
 #include "b200_games.h"
 #include "open_spiel/algorithms/mcts.h"
+#include "open_spiel/algorithms/minimax.h"
 #include "open_spiel/policy.h"
 #include "open_spiel/spiel.h"
 #include "open_spiel/spiel_bots.h"
@@ -54,6 +55,13 @@ class B200MCTSBot : public Bot {
   uint64_t steps_ = 0;
   Action last_best_ = kInvalidAction;
 };
+
+// algorithms::AlphaBetaSearch (minimax.h) with the reference's signature.  With no value function, on a game the device search
+// serves (b2s_alpha_beta_search: the deterministic b200 games except go 10..19), the root is copied to a one-lane batch and
+// solved on the device; reaching depth 0 at a non-terminal state, or kInvalidPlayer on a terminal root, is SpielFatalError as
+// in the reference.  Every other call (a value function, any other game) is the stock algorithms::AlphaBetaSearch.
+std::pair<double, Action> AlphaBetaSearch(const Game& game, const State* state, std::function<double(const State&)> value_function,
+                                          int depth_limit, Player maximizing_player, bool use_undo = true);
 
 class B200CFRSolver {
  public:

@@ -59,6 +59,9 @@ struct Batch {
   void* mcts_work = nullptr; u64* mcts_hist = nullptr; long long mcts_work_cap = 0;
   double* mcts_log = nullptr; int mcts_log_n = 0;
   void* mcts_pool = nullptr; unsigned long long mcts_pool_bytes = 0; unsigned long long* mcts_top = nullptr;
+  // AlphaBetaSearch scratch (b2s_alpha_beta_search): the roots in the lane-blob form, the frame stacks, the root counter
+  void* ab_work = nullptr; u64* ab_hist = nullptr; long long ab_work_cap = 0;
+  void* ab_stack = nullptr; size_t ab_stack_bytes = 0; unsigned long long* ab_next = nullptr;
   Ctx ctx() const { Ctx c; c.planes = planes; c.cap = cap; c.hist = hist; c.err = err; return c; }
   ~Batch() {
     for (auto& g : host_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
@@ -74,6 +77,8 @@ struct Batch {
     if (mcts_log) cudaFree(mcts_log);
     if (mcts_pool) cudaFree(mcts_pool);
     if (mcts_top) cudaFree(mcts_top);
+    for (void* p : {ab_work, (void*)ab_hist, ab_stack, (void*)ab_next})
+      if (p) cudaFree(p);
     delete ops;
   }
 };
@@ -796,6 +801,54 @@ int b2s_mcts_search(void* roots_batch, int64_t n_trees, const b2s_mcts_config* c
   if (int r = post()) return r;
   CU(cudaStreamSynchronize(st));          // the search is a long-running call; results are ready on return
   return 0;
+}
+
+int b2s_alpha_beta_search(void* roots_batch, int64_t n, const b2s_alpha_beta_config* cfg, double* value_d, int32_t* best_action_d,
+                          int64_t* nodes_d, uint8_t* status_d, void* stream) {
+  if (int r = check(roots_batch, n)) return r;
+  if (!cfg) return fail("alpha_beta: null config");
+  if (cfg->maximizing_player < -1 || cfg->maximizing_player > 1) return fail("alpha_beta: maximizing_player must be -1, 0 or 1");
+  if (cfg->max_nodes_per_root < 0) return fail("alpha_beta: negative max_nodes_per_root");
+  Batch* B = (Batch*)roots_batch;
+  size_t frame_bytes = 0;
+  long long resident = 0;
+  if (const char* e = B->ops->alpha_beta_limits(&frame_bytes, &resident)) return fail(e);
+  if (n == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  // one thread per root up to what the device holds at once and what B2S_ALPHA_BETA_STACK_BYTES of frame stacks allow
+  const unsigned long long frames = (unsigned long long)B->info.max_game_length + 2, per_thread = frames * frame_bytes;
+  long long threads = (n + 127) / 128 * 128;
+  if (threads > resident) threads = resident;
+  const long long fit = (long long)(B2S_ALPHA_BETA_STACK_BYTES / per_thread) / 128 * 128;
+  if (threads > fit) threads = fit;
+  if (threads < 128) threads = 128;
+  const size_t stack_bytes = (size_t)(per_thread * (unsigned long long)threads);
+  if (B->ab_stack_bytes < stack_bytes) {
+    if (B->ab_stack) cudaFree(B->ab_stack);
+    B->ab_stack = nullptr; B->ab_stack_bytes = 0;
+    CU(cudaMalloc(&B->ab_stack, stack_bytes));
+    B->ab_stack_bytes = stack_bytes;
+  }
+  if (B->ab_work_cap < n) {
+    if (B->ab_work) cudaFree(B->ab_work);
+    if (B->ab_hist) cudaFree(B->ab_hist);
+    B->ab_work = nullptr; B->ab_hist = nullptr; B->ab_work_cap = 0;
+    CU(cudaMalloc(&B->ab_work, (size_t)B->info.state_bytes * (size_t)n));
+    if (B->info.history_bytes) CU(cudaMalloc((void**)&B->ab_hist, (size_t)B->info.history_bytes * (size_t)n));
+    B->ab_work_cap = n;
+  }
+  if (!B->ab_next) CU(cudaMalloc((void**)&B->ab_next, sizeof(unsigned long long)));
+  Ctx work;
+  work.planes = B->ab_work; work.cap = B->ab_work_cap; work.hist = B->ab_hist; work.err = B->err;
+  B->ops->copy_to_blob(work, B->ctx(), n, st);
+  CU(cudaMemsetAsync(B->ab_next, 0, sizeof(unsigned long long), st));
+  AlphaBetaArgs a;
+  memset(&a, 0, sizeof a);
+  a.depth_limit = cfg->depth_limit; a.maximizing_player = cfg->maximizing_player; a.max_nodes = cfg->max_nodes_per_root;
+  a.threads = threads; a.stack = B->ab_stack; a.next = B->ab_next;
+  a.value = value_d; a.best_action = best_action_d; a.nodes = (long long*)nodes_d; a.status = status_d; a.err = B->err;
+  B->ops->alpha_beta(work, n, a, st);
+  return post();
 }
 
 }  // extern "C"

@@ -678,6 +678,10 @@ struct GameOps {
   virtual const char* mcts_eval_limits(int* max_legal, int* max_path) const = 0;
   virtual void mcts_eval_step(const Ctx& roots, const Ctx& leaves, long long n, const struct MctsEvalArgs& args, cudaStream_t) = 0;
   virtual void mcts_eval_report(long long n, const struct MctsEvalArgs& args, cudaStream_t) = 0;
+  // AlphaBetaSearch (alpha_beta.cuh): the bytes of one stack frame and the threads of k_alpha_beta the device holds at once, or
+  // an error string when the game is not served; the search of roots [0, n) of `work` (lane-blob form) on args.threads threads
+  virtual const char* alpha_beta_limits(size_t* frame_bytes, long long* resident_threads) const = 0;
+  virtual void alpha_beta(const Ctx& work, long long n, const struct AlphaBetaArgs& args, cudaStream_t) = 0;
   b2s_game_info info;
 };
 
@@ -798,12 +802,43 @@ struct GameOpsT : GameOps {
   const char* mcts_eval_limits(int* max_legal, int* max_path) const override;
   void mcts_eval_step(const Ctx& roots, const Ctx& leaves, long long n, const MctsEvalArgs& args, cudaStream_t st) override;
   void mcts_eval_report(long long n, const MctsEvalArgs& args, cudaStream_t st) override;
+  const char* alpha_beta_limits(size_t* frame_bytes, long long* resident_threads) const override;
+  void alpha_beta(const Ctx& work, long long n, const AlphaBetaArgs& args, cudaStream_t st) override;
 };
 
 }  // namespace b2s
 #include "mcts.cuh"
 #include "mcts_eval.cuh"
+#include "alpha_beta.cuh"
 namespace b2s {
+template <class R>
+const char* GameOpsT<R>::alpha_beta_limits(size_t* frame_bytes, long long* resident_threads) const {
+  if constexpr (ab_served<R>()) {
+    if (info.max_game_length + 2 > R::kMaxPath) return "alpha_beta: max_game_length too large for the device search stack";
+    int dev = 0, sms = 0, blocks = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, k_alpha_beta<R>, 128, 0) != cudaSuccess)
+      return "alpha_beta: cannot query the device's occupancy";
+    *frame_bytes = sizeof(AbFrame<R>);
+    *resident_threads = (long long)sms * blocks * 128;
+    return nullptr;
+  } else if constexpr (R::kMaxPath == 0) {
+    return "alpha_beta: AlphaBetaSearch needs a deterministic game (kuhn_poker and leduc_poker have chance nodes)";
+  } else {
+    return "alpha_beta: go 10..19 is not served (its search stack exceeds B2S_ALPHA_BETA_THREAD_STACK_BYTES per thread)";
+  }
+}
+template <class R>
+void GameOpsT<R>::alpha_beta(const Ctx& work, long long n, const AlphaBetaArgs& args, cudaStream_t st) {
+  if constexpr (ab_served<R>()) {
+    if (n <= 0) return;
+    AlphaBetaArgs a = args;
+    a.mask_words = info.mask_words;
+    k_alpha_beta<R><<<(unsigned)(a.threads / 128), 128, 0, st>>>(work, cfg, a, n);
+    ++g_launches;
+  }
+}
+
 template <class R>
 const char* GameOpsT<R>::mcts(const Ctx& roots, const Ctx& work, long long n, const MctsArgs& args, cudaStream_t st) {
   if constexpr (R::kMaxPath > 0) {

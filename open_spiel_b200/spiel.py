@@ -621,6 +621,28 @@ def mcts_search(batch, max_simulations, uct_c=2.0, n_rollouts=1, solve=True, see
     return out
 
 
+def alpha_beta_search(batch, depth_limit=-1, maximizing_player=-1, max_nodes=0, n=None):
+    """algorithms::AlphaBetaSearch (algorithms/minimax.cc:221-258) with no value function, from each of the first n lanes of
+    `batch` (b2s_alpha_beta_search).  Returns a dict of device tensors [n]: value float64 (PlayerReturn(maximizing_player) of
+    the solved root), best_action int32 (-1 for a terminal root), nodes int64 (child states generated) and status uint8
+    (0 solved, 1 max_nodes ran out, 2 a non-terminal state at depth 0, 3 maximizing_player -1 on a terminal root).
+    maximizing_player -1 is the root's current player; depth_limit -1 and max_nodes 0 are unlimited.  Enqueued on the
+    current stream."""
+    from ._lib import AlphaBetaConfig
+    n = batch.n if n is None else int(n)
+    dev = batch._dev
+    out = {
+        "value": torch.empty((n,), dtype=torch.float64, device=dev),
+        "best_action": torch.empty((n,), dtype=torch.int32, device=dev),
+        "nodes": torch.empty((n,), dtype=torch.int64, device=dev),
+        "status": torch.empty((n,), dtype=torch.uint8, device=dev),
+    }
+    cfg = AlphaBetaConfig(int(depth_limit), int(maximizing_player), int(max_nodes))
+    check(lib().b2s_alpha_beta_search(batch._h, n, C.byref(cfg), out["value"].data_ptr(), out["best_action"].data_ptr(),
+                                      out["nodes"].data_ptr(), out["status"].data_ptr(), batch._stream()))
+    return out
+
+
 class MCTSEvalSearch:
     """MCTSBot.MCTSearch (algorithms/mcts.cc:353-467) with a caller-supplied evaluator over n roots at once, driven in rounds
     (b2s_mcts_eval_*): every step() advances all live trees until each needs an evaluation or finishes; the states to evaluate
