@@ -392,6 +392,37 @@ typedef struct b2s_alpha_beta_config {
 int b2s_alpha_beta_search(void* roots_batch, int64_t n, const b2s_alpha_beta_config* cfg, double* value_d,
                           int32_t* best_action_d, int64_t* nodes_d, uint8_t* status_d, void* stream);
 
+/* algorithms::AlphaBetaSearch(game, state, value_function, depth_limit, maximizing_player) (minimax.cc:49-137, 221-258) with a
+ * caller-supplied value function, from each of lanes [0, n) of roots_batch, driven in rounds like b2s_mcts_eval_*.  The search is
+ * b2s_alpha_beta_search's (ascending actions, strict updates, std::max(alpha, value) / std::min(beta, value), cut at
+ * alpha >= beta, root at (-inf, +inf), maximizing_player -1 = the root's mover), except that a non-terminal state at depth 0
+ * takes value_function(state), "the value of the maximizing player": column maxp of the caller's [num_players] answer for it.  A
+ * terminal state is scored with Returns()[maxp] before the depth test, so terminal states are never sent to the caller; a
+ * non-terminal root with depth_limit 0 is itself the one evaluated state (best action -1).  Values are arbitrary doubles compared
+ * as IEEE does (a NaN child is never taken, -0.0 and +0.0 tie, +-inf work; all children at -inf leave best action -1) and passed
+ * through unchanged, bit for bit.
+ *   create   copies the roots (the roots batch may be reused at once) and their superko histories (go) into leaves_batch, which the
+ *            search owns until it is destroyed: same game, parameters and device, capacity >= n.  The caller must not change it
+ *            between steps.  One frame stack of min(depth_limit, max_game_length + 1) + 1 frames per root (max_game_length + 2 for
+ *            depth_limit < 0) is allocated here; a stack above B2S_ALPHA_BETA_THREAD_STACK_BYTES per root is an error (go 19x19
+ *            unlimited; go 10..19 is served at small depth limits), as are kuhn_poker and leduc_poker and a failed allocation.
+ *   step     advances every live root until it needs one value or finishes.  A root that needs one writes the state into its lane
+ *            i of leaves_batch (go: with the root's history plus the path's moves, so b2s_observation / b2s_legal_mask see the
+ *            real state) and sets pending_d[i] = 1 (nullable; n bytes); *n_pending_h (nullable, synchronises) counts them.  The
+ *            next step reads values_d[i * num_players + maxp] for each lane that was pending (values_d may be NULL on the first
+ *            step only).  One state per root and round: the caller sees exactly the reference's value_function calls, in order.
+ *   results  (device, nullable, lane i; final once a step has reported 0 pending): value_d double, best_action_d int32, nodes_d
+ *            int64 (child states generated), status_d uint8 (0 solved; 1 the budget max_nodes_per_root ran out, value NaN and best
+ *            action -1; 3 maximizing_player -1 on a terminal root, counted by b2s_error_count on leaves_batch; 2 cannot occur) and
+ *            evaluations_d int64 (value-function calls).
+ * Enqueued on `stream`; calls on one search must be ordered on the device. */
+int  b2s_alpha_beta_eval_create(void* roots_batch, int64_t n, const b2s_alpha_beta_config* cfg, void* leaves_batch,
+                                void** out_search, void* stream);
+int  b2s_alpha_beta_eval_step(void* search, const double* values_d, uint8_t* pending_d, int64_t* n_pending_h, void* stream);
+int  b2s_alpha_beta_eval_results(void* search, double* value_d, int32_t* best_action_d, int64_t* nodes_d, uint8_t* status_d,
+                                 int64_t* evaluations_d, void* stream);
+void b2s_alpha_beta_eval_destroy(void* search);
+
 /* ---- CFR ----------------------------------------------------------------------------------- */
 
 /* Replaces algorithms::CFRSolver / CFRPlusSolver (open_spiel/algorithms/cfr.h:312-357) for two-player

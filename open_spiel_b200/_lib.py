@@ -117,6 +117,10 @@ SIGNATURES = {
     "b2s_mcts_eval_results": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "b2s_mcts_eval_destroy": (None, [_VP]),
     "b2s_alpha_beta_search": (C.c_int, [_VP, _I64, C.POINTER(AlphaBetaConfig), _VP, _VP, _VP, _VP, _VP]),
+    "b2s_alpha_beta_eval_create": (C.c_int, [_VP, _I64, C.POINTER(AlphaBetaConfig), _VP, C.POINTER(_VP), _VP]),
+    "b2s_alpha_beta_eval_step": (C.c_int, [_VP, _VP, _VP, C.POINTER(_I64), _VP]),
+    "b2s_alpha_beta_eval_results": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "b2s_alpha_beta_eval_destroy": (None, [_VP]),
     "b2s_cfr_create": (C.c_int, [C.c_int, C.POINTER(Params), C.c_int, C.c_int, C.POINTER(_VP)]),
     "b2s_cfr_destroy": (None, [_VP]),
     "b2s_cfr_iterate": (C.c_int, [_VP, C.c_int, _VP]),

@@ -10,6 +10,7 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "batch_kernels.cuh"
@@ -982,6 +983,135 @@ int b2s_mcts_eval_results(void* search, int32_t* visit_counts_d, double* total_r
 }
 
 void b2s_mcts_eval_destroy(void* search) { delete (MctsEvalSearch*)search; }
+
+}  // extern "C"
+
+// ---- AlphaBetaSearch with a caller-supplied value function (alpha_beta.cuh) ---------------------------------------------------
+namespace b2s {
+struct AlphaBetaEvalSearch {
+  Batch* leaves = nullptr;
+  long long n = 0;
+  int steps = 0;
+  AlphaBetaEvalArgs a;
+  void* roots = nullptr;            // the roots in the lane-blob form, leaves->cap lanes (lanes [0, n) used)
+  void* stack = nullptr;            // [frames][n] AbFrame<R, double>
+  AbEvalRoot* ctx = nullptr;
+  unsigned char* pending = nullptr;
+  unsigned long long* n_pending = nullptr;
+  double* value = nullptr;
+  int* best_action = nullptr;
+  long long* nodes = nullptr;
+  unsigned char* status = nullptr;
+  long long* evals = nullptr;
+  ~AlphaBetaEvalSearch() {
+    if (leaves) cudaSetDevice(leaves->device);
+    for (void* p : {roots, stack, (void*)ctx, (void*)pending, (void*)n_pending, (void*)value, (void*)best_action, (void*)nodes,
+                    (void*)status, (void*)evals})
+      if (p) cudaFree(p);
+  }
+  Ctx roots_ctx() const { Ctx c; c.planes = roots; c.cap = leaves->cap; c.hist = leaves->hist; c.err = leaves->err; return c; }
+};
+}  // namespace b2s
+
+extern "C" {
+
+int b2s_alpha_beta_eval_create(void* roots_batch, int64_t n, const b2s_alpha_beta_config* cfg, void* leaves_batch, void** out_search,
+                               void* stream) {
+  if (!out_search) return fail("alpha_beta_eval: null out_search");
+  *out_search = nullptr;
+  if (int r = check(roots_batch, n)) return r;
+  if (!cfg || !leaves_batch) return fail("alpha_beta_eval: null argument");
+  Batch* B = (Batch*)roots_batch;
+  Batch* L = (Batch*)leaves_batch;
+  if (L->device != B->device || memcmp(&L->info, &B->info, sizeof(b2s_game_info)) != 0)
+    return fail("alpha_beta_eval: the leaves batch must be of the same game, parameters and device as the roots batch");
+  if (n < 1) return fail("alpha_beta_eval: n must be >= 1");
+  if (L->cap < n) return fail("alpha_beta_eval: the leaves batch holds fewer lanes than n");
+  if (cfg->maximizing_player < -1 || cfg->maximizing_player > 1) return fail("alpha_beta_eval: maximizing_player must be -1, 0 or 1");
+  if (cfg->max_nodes_per_root < 0) return fail("alpha_beta_eval: negative max_nodes_per_root");
+  size_t frame_bytes = 0;
+  if (const char* e = B->ops->alpha_beta_eval_limits(&frame_bytes)) return fail(e);
+  // the deepest node that saves a frame is at depth min(depth_limit, max_game_length + 1) - 1; one more frame as the exact search
+  const long long len = B->info.max_game_length;
+  const long long frames = cfg->depth_limit < 0 ? len + 2 : (cfg->depth_limit < len + 1 ? cfg->depth_limit : len + 1) + 1;
+  const unsigned long long per_root = (unsigned long long)frames * frame_bytes;
+  if (per_root > B2S_ALPHA_BETA_THREAD_STACK_BYTES) {
+    char msg[256];
+    snprintf(msg, sizeof msg, "alpha_beta_eval: %lld frames of %zu bytes per root exceed B2S_ALPHA_BETA_THREAD_STACK_BYTES (%u): lower "
+             "depth_limit", frames, frame_bytes, (unsigned)B2S_ALPHA_BETA_THREAD_STACK_BYTES);
+    return fail(msg);
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  std::unique_ptr<AlphaBetaEvalSearch> S(new AlphaBetaEvalSearch);
+  S->leaves = L; S->n = n;
+  const size_t N = (size_t)n;
+  CU(cudaMalloc(&S->roots, (size_t)B->info.state_bytes * (size_t)L->cap));
+  CU(cudaMalloc(&S->stack, (size_t)per_root * N));
+  CU(cudaMalloc((void**)&S->ctx, sizeof(AbEvalRoot) * N));
+  CU(cudaMalloc((void**)&S->pending, N));
+  CU(cudaMalloc((void**)&S->n_pending, sizeof(unsigned long long)));
+  CU(cudaMalloc((void**)&S->value, sizeof(double) * N));
+  CU(cudaMalloc((void**)&S->best_action, sizeof(int) * N));
+  CU(cudaMalloc((void**)&S->nodes, sizeof(long long) * N));
+  CU(cudaMalloc((void**)&S->status, N));
+  CU(cudaMalloc((void**)&S->evals, sizeof(long long) * N));
+  CU(cudaMemsetAsync(S->ctx, 0, sizeof(AbEvalRoot) * N, st));   // phase kAbEvalInit
+  CU(cudaMemsetAsync(S->pending, 0, N, st));
+  for (auto& z : {std::make_pair((void*)S->value, sizeof(double)), std::make_pair((void*)S->best_action, sizeof(int)),
+                  std::make_pair((void*)S->nodes, sizeof(long long)), std::make_pair((void*)S->status, (size_t)1),
+                  std::make_pair((void*)S->evals, sizeof(long long))})
+    CU(cudaMemsetAsync(z.first, 0, z.second * N, st));
+  // roots -> blob lanes of the search; their superko histories (go) -> the leaves batch, where the search extends them
+  B->ops->copy_to_blob(S->roots_ctx(), B->ctx(), n, st);
+  if (int r = post()) return r;
+  AlphaBetaEvalArgs& a = S->a;
+  memset(&a, 0, sizeof a);
+  a.depth_limit = cfg->depth_limit; a.maximizing_player = cfg->maximizing_player; a.max_nodes = cfg->max_nodes_per_root;
+  a.stack = S->stack; a.roots = S->ctx; a.pending = S->pending; a.n_pending = S->n_pending;
+  a.value = S->value; a.best_action = S->best_action; a.nodes = S->nodes; a.status = S->status; a.evals = S->evals; a.err = L->err;
+  CU(cudaStreamSynchronize(st));
+  *out_search = S.release();
+  return 0;
+}
+
+int b2s_alpha_beta_eval_step(void* search, const double* values_d, uint8_t* pending_d, int64_t* n_pending_h, void* stream) {
+  if (!search) return fail("alpha_beta_eval: null search");
+  AlphaBetaEvalSearch* S = (AlphaBetaEvalSearch*)search;
+  if (S->steps > 0 && !values_d) return fail("alpha_beta_eval: values are required after the first step");
+  CU(cudaSetDevice(S->leaves->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  AlphaBetaEvalArgs a = S->a;
+  a.values = values_d;
+  CU(cudaMemsetAsync(S->n_pending, 0, sizeof(unsigned long long), st));
+  S->leaves->ops->alpha_beta_eval_step(S->roots_ctx(), S->leaves->ctx(), S->n, a, st);
+  if (int r = post()) return r;
+  ++S->steps;
+  if (pending_d) CU(cudaMemcpyAsync(pending_d, S->pending, (size_t)S->n, cudaMemcpyDeviceToDevice, st));
+  if (n_pending_h) {
+    unsigned long long v = 0;
+    CU(cudaMemcpyAsync(&v, S->n_pending, sizeof v, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    *n_pending_h = (int64_t)v;
+  }
+  return 0;
+}
+
+int b2s_alpha_beta_eval_results(void* search, double* value_d, int32_t* best_action_d, int64_t* nodes_d, uint8_t* status_d,
+                                int64_t* evaluations_d, void* stream) {
+  if (!search) return fail("alpha_beta_eval: null search");
+  AlphaBetaEvalSearch* S = (AlphaBetaEvalSearch*)search;
+  CU(cudaSetDevice(S->leaves->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t N = (size_t)S->n;
+  if (value_d) CU(cudaMemcpyAsync(value_d, S->value, sizeof(double) * N, cudaMemcpyDeviceToDevice, st));
+  if (best_action_d) CU(cudaMemcpyAsync(best_action_d, S->best_action, sizeof(int) * N, cudaMemcpyDeviceToDevice, st));
+  if (nodes_d) CU(cudaMemcpyAsync(nodes_d, S->nodes, sizeof(long long) * N, cudaMemcpyDeviceToDevice, st));
+  if (status_d) CU(cudaMemcpyAsync(status_d, S->status, N, cudaMemcpyDeviceToDevice, st));
+  if (evaluations_d) CU(cudaMemcpyAsync(evaluations_d, S->evals, sizeof(long long) * N, cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
+void b2s_alpha_beta_eval_destroy(void* search) { delete (AlphaBetaEvalSearch*)search; }
 
 }  // extern "C"
 

@@ -682,6 +682,10 @@ struct GameOps {
   // an error string when the game is not served; the search of roots [0, n) of `work` (lane-blob form) on args.threads threads
   virtual const char* alpha_beta_limits(size_t* frame_bytes, long long* resident_threads) const = 0;
   virtual void alpha_beta(const Ctx& work, long long n, const struct AlphaBetaArgs& args, cudaStream_t) = 0;
+  // AlphaBetaSearch with a caller-supplied value function (alpha_beta.cuh): the bytes of one frame of k_alpha_beta_eval_step, or an
+  // error string when the game is not served; one step of roots [0, n) (`roots` in the lane-blob form, `leaves` the caller's batch)
+  virtual const char* alpha_beta_eval_limits(size_t* frame_bytes) const = 0;
+  virtual void alpha_beta_eval_step(const Ctx& roots, const Ctx& leaves, long long n, const struct AlphaBetaEvalArgs& args, cudaStream_t) = 0;
   b2s_game_info info;
 };
 
@@ -804,6 +808,8 @@ struct GameOpsT : GameOps {
   void mcts_eval_report(long long n, const MctsEvalArgs& args, cudaStream_t st) override;
   const char* alpha_beta_limits(size_t* frame_bytes, long long* resident_threads) const override;
   void alpha_beta(const Ctx& work, long long n, const AlphaBetaArgs& args, cudaStream_t st) override;
+  const char* alpha_beta_eval_limits(size_t* frame_bytes) const override;
+  void alpha_beta_eval_step(const Ctx& roots, const Ctx& leaves, long long n, const AlphaBetaEvalArgs& args, cudaStream_t st) override;
 };
 
 }  // namespace b2s
@@ -835,6 +841,26 @@ void GameOpsT<R>::alpha_beta(const Ctx& work, long long n, const AlphaBetaArgs& 
     AlphaBetaArgs a = args;
     a.mask_words = info.mask_words;
     k_alpha_beta<R><<<(unsigned)(a.threads / 128), 128, 0, st>>>(work, cfg, a, n);
+    ++g_launches;
+  }
+}
+template <class R>
+const char* GameOpsT<R>::alpha_beta_eval_limits(size_t* frame_bytes) const {
+  if constexpr (R::kMaxPath > 0) {
+    *frame_bytes = sizeof(AbFrame<R, double>);
+    return nullptr;
+  } else {
+    return "alpha_beta_eval: AlphaBetaSearch needs a deterministic game (kuhn_poker and leduc_poker have chance nodes)";
+  }
+}
+template <class R>
+void GameOpsT<R>::alpha_beta_eval_step(const Ctx& roots, const Ctx& leaves, long long n, const AlphaBetaEvalArgs& args, cudaStream_t st) {
+  if constexpr (R::kMaxPath > 0) {
+    if (n <= 0) return;
+    AlphaBetaEvalArgs a = args;
+    a.mask_words = info.mask_words;
+    a.num_players = info.num_players;
+    k_alpha_beta_eval_step<R><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(roots, leaves, cfg, a, n);
     ++g_launches;
   }
 }

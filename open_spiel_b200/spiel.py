@@ -749,6 +749,86 @@ def mcts_search_evaluated(batch, evaluate, max_simulations, uct_c=2.0, solve=Tru
     return out
 
 
+class AlphaBetaEvalSearch:
+    """algorithms::AlphaBetaSearch (algorithms/minimax.cc:49-137, 221-258) with a caller-supplied value function over n roots
+    at once, driven in rounds (b2s_alpha_beta_eval_*): every step() advances all live roots until each needs one value or
+    finishes; the states to evaluate are lanes of `.leaves` (a BatchedState of the roots' game), flagged by the returned
+    `pending` mask.  The next step() takes their values: a float64 device tensor [n, num_players] whose column maxp is the
+    reference's value_function(state), the value of the maximizing player (the shape mcts_search_evaluated's values have).
+    step(None) starts the search.  The evaluated states and their order are the reference's value_function calls; terminal
+    states are never evaluated.  depth_limit -1 is unlimited, maximizing_player -1 the root's mover, max_nodes 0 no budget."""
+
+    def __init__(self, roots_batch, depth_limit, maximizing_player=-1, max_nodes=0, n=None, leaves=None):
+        from ._lib import AlphaBetaConfig
+        self._h = C.c_void_p()
+        self.n = roots_batch.n if n is None else int(n)
+        self.info = roots_batch.info
+        self._dev = roots_batch._dev
+        self.leaves = leaves if leaves is not None else BatchedState(roots_batch.game, self.n, roots_batch.device)
+        cfg = AlphaBetaConfig(int(depth_limit), int(maximizing_player), int(max_nodes))
+        check(lib().b2s_alpha_beta_eval_create(roots_batch._h, self.n, C.byref(cfg), self.leaves._h, C.byref(self._h),
+                                               self.leaves._stream()))
+        self._pending = torch.zeros((self.n,), dtype=torch.uint8, device=self._dev)
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib().b2s_alpha_beta_eval_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def step(self, values=None):
+        """One round.  Returns (pending [n] bool tensor, number of pending lanes); 0 pending = the search is over."""
+        ptr = None
+        if values is not None:
+            width = self.info.num_players
+            if values.dtype != torch.float64 or not values.is_cuda or values.dim() != 2 or values.shape[0] < self.n or \
+                    values.shape[1] != width:
+                raise B2SError("alpha_beta_eval: values must be a float64 CUDA tensor of shape [n, %d]" % width)
+            if not values.is_contiguous():
+                raise B2SError("alpha_beta_eval: values must be contiguous")
+            ptr = values.data_ptr()
+        n_pending = C.c_int64()
+        check(lib().b2s_alpha_beta_eval_step(self._h, ptr, self._pending.data_ptr(), C.byref(n_pending), self.leaves._stream()))
+        return self._pending.bool(), n_pending.value
+
+    def results(self):
+        """dict of device tensors [n]: value float64, best_action int32 (-1 for a terminal root or a depth-0 root), nodes int64
+        (child states generated), status uint8 (0 solved, 1 max_nodes ran out, 3 maximizing_player -1 on a terminal root) and
+        evaluations int64 (value-function calls).  Final once step() has reported 0 pending."""
+        n, dev = self.n, self._dev
+        out = {
+            "value": torch.empty((n,), dtype=torch.float64, device=dev),
+            "best_action": torch.empty((n,), dtype=torch.int32, device=dev),
+            "nodes": torch.empty((n,), dtype=torch.int64, device=dev),
+            "status": torch.empty((n,), dtype=torch.uint8, device=dev),
+            "evaluations": torch.empty((n,), dtype=torch.int64, device=dev),
+        }
+        check(lib().b2s_alpha_beta_eval_results(self._h, *[out[k].data_ptr() for k in ("value", "best_action", "nodes", "status",
+                                                                                        "evaluations")], self.leaves._stream()))
+        return out
+
+
+def alpha_beta_search_evaluated(batch, value_function, depth_limit, maximizing_player=-1, max_nodes=0, n=None, leaves=None):
+    """Batched AlphaBetaSearch with a caller-supplied batched value function: `value_function(leaves, pending)` gets the leaves
+    BatchedState and the pending mask (device tensors) and returns values [n, num_players] for the pending lanes (column maxp
+    is the maximizing player's value; other float dtypes are converted).  Runs the rounds until every root has finished and
+    returns AlphaBetaEvalSearch.results() plus "rounds" (value_function calls)."""
+    search = AlphaBetaEvalSearch(batch, depth_limit, maximizing_player, max_nodes, n, leaves)
+    values = None
+    rounds = 0
+    while True:
+        pending, n_pending = search.step(values)
+        if n_pending == 0:
+            break
+        rounds += 1
+        values = value_function(search.leaves, pending).to(torch.float64).contiguous()
+    out = search.results()
+    out["rounds"] = rounds
+    return out
+
+
 def dirichlet_noise(batch, alpha, generator=None, n=None):
     """Per lane a Dirichlet(alpha) vector over the lane's legal actions, scattered by action id ([n, A] float64, zero on illegal
     actions): the noise dirichlet_noise (algorithms/mcts.cc:188-203) draws for the root, here drawn in torch as normalised
