@@ -778,7 +778,10 @@ struct GameOpsT : GameOps {
     launch(k_step_compact_zc<R, R::kIlp>, n, R::kIlp, st, c, cfg, a_host, status_host, small_mask(), n);
   }
   void rollout(const Ctx& c, u64 seed, long long lane_offset, float* rets, int* plies, long long n, cudaStream_t st) override {
-    launch(k_rollout<R>, n, 1, st, c, cfg, seed, lane_offset, info.mask_words, info.max_game_length + 4, rets, plies, n);
+    // max_game_length counts the players' moves only (kuhn_poker.h:121, leduc_poker.h:233-241); the poker games add up to
+    // num_players + 1 chance plies (5-player kuhn_poker: 5 deals + 9 moves = 14 plies), so the cap leaves room for them
+    launch(k_rollout<R>, n, 1, st, c, cfg, seed, lane_offset, info.mask_words, info.max_game_length + info.num_players + 4, rets,
+           plies, n);
   }
   void copy(const Ctx& dst, long long dst0, const Ctx& src, long long src0, int src_step, long long count, cudaStream_t st) override {
     launch(k_copy<R>, count, 1, st, dst, dst0, src, src0, src_step, count, cfg);

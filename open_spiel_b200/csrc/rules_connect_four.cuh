@@ -49,6 +49,7 @@ struct ConnectFourCore {
     int rgather;       // 1: row extraction (bits c*h1 -> bits 0..cols-1) by multiply-gather, verified on the host
     u32 rmul_lo, rmul_hi;
     int rsh_lo, rsh_hi, rcols_lo, rfirst_hi;
+    int line4;         // 1: has_line's four-in-a-row fast path (k == 4, every shift below 64); sits in padding before top
     u64 top;           // top playable cell of every column
     u64 board;         // all playable cells
     u64 bottom;        // bit c*h1 of every column (row 0)
@@ -77,6 +78,7 @@ struct ConnectFourCore {
     if (kStd && (c.rows != kStdRows || c.cols != kStdCols || c.k != kStdK)) return "connect_four: not the default board";
     c.h1 = c.rows + 1;
     c.meta = (c.rows + 1) * c.cols <= 62 ? 1 : 0;
+    c.line4 = c.k == 4 && 2 * (c.h1 + 1) < 64 ? 1 : 0;
     c.top = 0; c.board = 0; c.bottom = 0;
     for (int col = 0; col < c.cols; ++col) {
       c.top |= 1ull << (col * c.h1 + c.rows - 1);
@@ -167,7 +169,9 @@ struct ConnectFourCore {
   }
 
   __device__ static __forceinline__ bool has_line(u64 b, const Cfg& c) {
-    if (K(c) == 4) {
+    // four in a row by three shift-and-steps; its largest shift, 2 * (h1 + 1), must stay below 64 (a shift by 64 or more is
+    // undefined in C++: the host build gives wrong lines there), so boards of 30 rows and more take the guarded loop
+    if (kStd || c.line4) {
       const int d1 = H1(c), d2 = H1(c) + 1, d3 = H1(c) - 1;
       u64 m1 = b & (b >> 1), m2 = b & (b >> d1), m3 = b & (b >> d2), m4 = b & (b >> d3);
       u64 any = (m1 & (m1 >> 2)) | (m2 & (m2 >> (2 * d1))) | (m3 & (m3 >> (2 * d2))) | (m4 & (m4 >> (2 * d3)));

@@ -36,7 +36,9 @@ struct HexRules {
     c.rows = p.rows >= 0 ? p.rows : bs;
     c.swap = p.swap > 0 ? 1 : 0;
     c.plain = p.plain_obs_tensor > 0 ? 1 : 0;
-    if (c.cols < 2 || c.rows < 1) return "hex: board too small";
+    // one row or one column: the reference's edge tests (hex.cc:122-126, 146-150) give a stone on both edges only one of them,
+    // so no game ever ends and a full board is a non-terminal state with no legal action
+    if (c.cols < 2 || c.rows < 2) return "hex: board too small (num_rows and num_cols must be at least 2)";
     if (c.cols * c.rows > 121 || c.cols > 63) return "hex: at most 121 cells on the device path";
     if (c.plain && c.cols < c.rows) return "hex: plain_obs_tensor with num_cols < num_rows is not supported (the reference indexes out of its plane)";
     if (c.swap && c.cols > c.rows)
