@@ -258,6 +258,8 @@ void B200CFRSolver::Import(const Tables& t) {
   Check(b2s_stream_synchronize(0, nullptr));
 }
 
+B200CFRBRSolver::B200CFRBRSolver(const Game& game) : B200CFRSolver(game, false, B2S_CFR_BEST_RESPONSE_OPPONENTS) {}
+
 B200MCCFRSolver::B200MCCFRSolver(const Game& game, Kind kind, uint64_t seed, bool full_average, double epsilon, int per_update)
     : B200CFRSolver(game, false, B2S_CFR_MCCFR_TABLES), kind_(kind), seed_(seed), full_average_(full_average), epsilon_(epsilon),
       per_update_(per_update < 1 ? 1 : per_update) {}

@@ -2,6 +2,7 @@
 // OpenSpiel code switches by changing a type name:
 //   B200MCTSBot   : open_spiel::Bot           <- algorithms::MCTSBot (mcts.h:149-230) with a RandomRolloutEvaluator
 //   B200CFRSolver                             <- algorithms::CFRSolver / CFRPlusSolver (cfr.h:312-357)
+//   B200CFRBRSolver                           <- algorithms::CFRBRSolver (cfr_br.h)
 // Every computation is a call into the b2s C ABI (libb2s.so); these classes only translate between the reference's
 // host objects (State history, TabularPolicy keyed by information-state strings) and device batches / tables.
 #ifndef OPEN_SPIEL_B200_ADAPTER_B200_ALGORITHMS_H_
@@ -92,6 +93,14 @@ class B200CFRSolver {
   b2s_cfr_info info_;
   std::vector<std::string> keys_;                       // information-state string of every device table row
   std::vector<int32_t> offsets_, legal_;
+};
+
+// CFRBRSolver (cfr_br.h): each iteration both players' pure best responses to the current policy (the uniform policy on
+// iteration 1), each player's traversal against the other's best response, then regret matching; tables match the reference
+// bit for bit (B2S_CFR_BEST_RESPONSE_OPPONENTS).
+class B200CFRBRSolver : public B200CFRSolver {
+ public:
+  explicit B200CFRBRSolver(const Game& game);
 };
 
 // ExternalSamplingMCCFRSolver (external_sampling_mccfr.h:40-95) / OutcomeSamplingMCCFRSolver (outcome_sampling_mccfr.h:40-66,

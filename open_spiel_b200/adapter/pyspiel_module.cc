@@ -1,5 +1,5 @@
 // pyspiel-compatible Python module for the b2s path (pybind11): the surface SURVEY §8(b) lists —
-// pyspiel.load_game, Game, State, MCTSBot / RandomRolloutEvaluator / SearchNode, CFRSolver / CFRPlusSolver, policies,
+// pyspiel.load_game, Game, State, MCTSBot / RandomRolloutEvaluator / SearchNode, CFRSolver / CFRPlusSolver / CFRBRSolver, policies,
 // exploitability — over the unmodified reference library plus the B200 drop-ins, which this module registers over the
 // stock tic_tac_toe / connect_four / breakthrough / hex / go / kuhn_poker / leduc_poker at import time, so
 // `pyspiel.load_game("go(board_size=9)")` returns a B200Game.  Method names and argument orders are those of
@@ -358,6 +358,23 @@ PYBIND11_MODULE(pyspiel, m) {
             return solver;
           }));
   m.def("CFRPlusSolver", [](std::shared_ptr<Game> g) { return new b200::B200CFRSolver(*g, true); });
+  py::class_<b200::B200CFRBRSolver, b200::B200CFRSolver>(m, "CFRBRSolver")   // policy.cc:264-280
+      .def(py::init([](std::shared_ptr<Game> g) { return new b200::B200CFRBRSolver(*g); }))
+      .def(py::pickle(
+          [](const b200::B200CFRBRSolver& s) {
+            b200::B200CFRSolver::Tables t = s.Export();
+            return py::make_tuple(s.game().ToString(), t.iteration, t.regrets, t.cumulative_policy, t.current_policy);
+          },
+          [](py::tuple st) {
+            auto solver = std::make_unique<b200::B200CFRBRSolver>(*LoadGame(st[0].cast<std::string>()));
+            b200::B200CFRSolver::Tables t;
+            t.iteration = st[1].cast<int>();
+            t.regrets = st[2].cast<std::vector<double>>();
+            t.cumulative_policy = st[3].cast<std::vector<double>>();
+            t.current_policy = st[4].cast<std::vector<double>>();
+            solver->Import(t);
+            return solver;
+          }));
 
   // ---- MCCFR (python/pybind11/policy.cc:282-335 names; extra keyword: traversals / trajectories per update) ------------
   py::enum_<algorithms::AverageType>(m, "MCCFRAverageType")

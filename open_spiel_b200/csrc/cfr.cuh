@@ -20,8 +20,8 @@
 // The reference prunes decision nodes where every player's reach is 0 and returns zeros (cfr.cc:350-355);
 // we reproduce the returned zeros; the skipped updates below such a node add +-0 and change nothing.
 //
-// Files: cfr_tree.cu (tree construction, solver lifetime), cfr_full.cu (full-width CFR, NashConv / best response, sharded
-// NCCL path), cfr_mccfr.cu (external- and outcome-sampling MCCFR).
+// Files: cfr_tree.cu (tree construction, solver lifetime), cfr_full.cu (full-width CFR, CFR-BR, NashConv / best response,
+// sharded NCCL path), cfr_mccfr.cu (external- and outcome-sampling MCCFR).
 #pragma once
 #include <vector>
 
@@ -53,9 +53,10 @@ struct CfrDev {
   const int* policy_index;     // [n] index into cur_policy of the edge into n (-1 when the parent is a chance node)
   const signed char* par_actor;// [n] actor of the parent (0/1 player, 2 chance)
   const double* chance_reach;  // [n] the chance player's reach of n (product of chance probabilities along the path)
-  double* reach;               // [n][2]  (player 0, player 1); NashConv keeps the responder's counterfactual reach in slot 0
-  double* edge_prob;           // [n]
-  double* value;               // [n][2]
+  double* reach;               // [n][2]  (player 0, player 1); NashConv keeps the responder's counterfactual reach in slot 0;
+                               // [2][n][2] on a CFR-BR solver (one [n][2] block per traversal, cfr_level_passes<2>)
+  double* edge_prob;           // [n]; [2][n] on a CFR-BR solver
+  double* value;               // [n][2]; [2][n][2] on a CFR-BR solver
   double* regrets;             // [E]
   double* cum_policy;          // [E]
   double* cur_policy;          // [E]
@@ -82,46 +83,76 @@ __device__ __forceinline__ void regret_matching(const double* regrets, double* p
   }
 }
 
-// One traversal's tree passes, shared by the single-GPU kernel, the sharded one and MCCFR's full averaging: (1) edge
-// probabilities from the frozen policy, (2) L level steps in which the reach probabilities move one level DOWN while the
-// state values move one level UP.
-__device__ __forceinline__ void cfr_level_passes(const CfrDev& d, int tid, int nt) {
-  const int L = d.n_levels;
-  for (int n = 1 + tid; n < d.n_nodes; n += nt) {
+// The probability of the edge into node n under the frozen current policy: the policy at decision nodes, the chance
+// probability below chance nodes.  Traversal index t is unused: every traversal of plain CFR follows the same policy.
+struct CurrentPolicyEdge {
+  __device__ __forceinline__ double operator()(const CfrDev& d, int n, int) const {
     int pi = d.policy_index[n];
-    d.edge_prob[n] = pi >= 0 ? d.cur_policy[pi] : d.chance_prob[n];
+    return pi >= 0 ? d.cur_policy[pi] : d.chance_prob[n];
   }
-  if (tid == 0) { d.reach[0] = 1.0; d.reach[1] = 1.0; }
+};
+
+// T traversals' tree passes, shared by the single-GPU kernel, the sharded one, MCCFR's full averaging (T = 1) and CFR-BR
+// (T = 2): (1) edge probabilities edge(d, n, t) from the frozen policies, (2) L level steps in which the reach probabilities
+// move one level DOWN while the state values move one level UP.  Traversal t keeps its edge probabilities at
+// edge_prob[t * n ...], its reach and values at reach / value[2 * t * n ...] (n = number of nodes).
+template <int T = 1, class EdgeProb = CurrentPolicyEdge>
+__device__ __forceinline__ void cfr_level_passes(const CfrDev& d, int tid, int nt, EdgeProb edge = {}) {
+  const int L = d.n_levels, N = d.n_nodes;
+  for (int n = 1 + tid; n < N; n += nt) {
+#pragma unroll
+    for (int t = 0; t < T; ++t) d.edge_prob[t * N + n] = edge(d, n, t);
+  }
+  if (tid == 0) {
+#pragma unroll
+    for (int t = 0; t < T; ++t) { d.reach[2 * t * N] = 1.0; d.reach[2 * t * N + 1] = 1.0; }
+  }
   __syncthreads();
   for (int k = 0; k < L; ++k) {
     int ld = k + 1;                       // reach: new_reach_probabilities[current_player] *= prob (cfr.cc:457)
     if (ld < L) {
       for (int n = d.level_off[ld] + tid; n < d.level_off[ld + 1]; n += nt) {
         int par = d.parent[n];
-        double r0 = d.reach[2 * par], r1 = d.reach[2 * par + 1];
         int a = d.par_actor[n];
-        if (a == 0) r0 = __dmul_rn(r0, d.edge_prob[n]); else if (a == 1) r1 = __dmul_rn(r1, d.edge_prob[n]);
-        d.reach[2 * n] = r0; d.reach[2 * n + 1] = r1;
+#pragma unroll
+        for (int t = 0; t < T; ++t) {
+          double* reach = d.reach + 2 * t * N;
+          double r0 = reach[2 * par], r1 = reach[2 * par + 1];
+          if (a == 0) r0 = __dmul_rn(r0, d.edge_prob[t * N + n]); else if (a == 1) r1 = __dmul_rn(r1, d.edge_prob[t * N + n]);
+          reach[2 * n] = r0; reach[2 * n + 1] = r1;
+        }
       }
     }
     int lu = L - 1 - k;                   // values: state_value[i] += prob * child_value[i] (cfr.cc:461-463)
     for (int n = d.level_off[lu] + tid; n < d.level_off[lu + 1]; n += nt) {
-      double v0, v1;
-      if (d.kind[n] == 0) { v0 = d.ret[2 * n]; v1 = d.ret[2 * n + 1]; }
-      else {
-        v0 = 0.0; v1 = 0.0;
-        int fc = d.first_child[n];
-        for (int c = 0; c < d.nchild[n]; ++c) {
-          double pr = d.edge_prob[fc + c];
-          v0 = __dadd_rn(v0, __dmul_rn(pr, d.value[2 * (fc + c)]));
-          v1 = __dadd_rn(v1, __dmul_rn(pr, d.value[2 * (fc + c) + 1]));
+#pragma unroll
+      for (int t = 0; t < T; ++t) {
+        double* value = d.value + 2 * t * N;
+        const double* edge_prob = d.edge_prob + t * N;
+        double v0, v1;
+        if (d.kind[n] == 0) { v0 = d.ret[2 * n]; v1 = d.ret[2 * n + 1]; }
+        else {
+          v0 = 0.0; v1 = 0.0;
+          int fc = d.first_child[n];
+          for (int c = 0; c < d.nchild[n]; ++c) {
+            double pr = edge_prob[fc + c];
+            v0 = __dadd_rn(v0, __dmul_rn(pr, value[2 * (fc + c)]));
+            v1 = __dadd_rn(v1, __dmul_rn(pr, value[2 * (fc + c) + 1]));
+          }
         }
+        value[2 * n] = v0; value[2 * n + 1] = v1;
       }
-      d.value[2 * n] = v0; d.value[2 * n + 1] = v1;
     }
     __syncthreads();
   }
 }
+
+// CFR-BR's best-response scratch (a kernel argument of k_cfr_br only, so CfrDev and the other kernels stay as they are).
+struct CfrBrDev {
+  int* best;                   // [I] the pure best response at information state I, as an index into its legal actions
+  double* cf_reach;            // [n_hist] counterfactual reach of history slot hh for the player acting there
+  double* value;               // [2][n] best-response value of every node for responder 0, then responder 1
+};
 
 struct CfrSolver {
   // multi-GPU: communicator (owned or adopted), private stream + a CUDA graph of kGraphIters sharded iterations
@@ -141,6 +172,8 @@ struct CfrSolver {
   int game_id = 0;
   int iteration = 0;
   int linear_averaging = 0, rm_plus = 0;
+  int best_response_opponents = 0;                           // CFR-BR (B2S_CFR_BEST_RESPONSE_OPPONENTS): k_cfr_br, br scratch
+  CfrBrDev br{};
   int tensor_size = 0;
   CfrDev d;
   std::vector<void*> allocs;

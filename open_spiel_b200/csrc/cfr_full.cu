@@ -1,5 +1,6 @@
 // Full-width CFR (single-GPU persistent kernel and the sharded / NCCL iteration) and NashConv / best response on the
 // flattened tree of cfr_tree.cu.  Floating-point conventions: cfr.cuh.
+#include <float.h>
 #include <string.h>
 
 #include "cfr.cuh"
@@ -59,6 +60,109 @@ __global__ void __launch_bounds__(1024) k_cfr(CfrDev d, int iters, int iteration
       }
       __syncthreads();
     }
+  }
+}
+
+// ---- CFR-BR (algorithms/cfr_br.cc:50-82, CFRBRSolver::EvaluateAndUpdatePolicy) ------------------------------------
+// Per iteration: (1) the pure best response BR_b of each player b to the current policy (the uniform policy on iteration 1,
+// when the reference's best-response computers still hold the UniformPolicy they were built with); (2) for p = 0, 1 the
+// traversal ComputeCounterFactualRegret(root, p) with the other player replaced by its best response as a 1.0 / 0.0 policy,
+// updating p's regrets and (plain) average policy; (3) regret matching of the whole table.  Both best responses answer the
+// same frozen policy and neither traversal reads what the other writes, so both responders share one bottom-up sweep and
+// both traversals one set of level steps (cfr_level_passes<2>): L + (L + 1) + 1 barriers per iteration, where k_cfr has
+// 2 (L + 2).
+//
+// The best response follows TabularBestResponse (best_response.cc:79-228, history_tree.cc:160-240; prob_cut_threshold and
+// action_value_tolerance at their defaults of -1) operation for operation, every product and sum explicitly rounded:
+//   counterfactual reach of a history h of responder b (DecisionNodes): formed from h UPWARD, acc = q * acc from 1.0, with
+//     q = the chance probability, the evaluated policy at the other player's nodes, nothing (1.0) at b's own nodes;
+//   action value at an information state: sum over its histories in DFS order (GetAllInfoSets) of cf_reach * V(child), from
+//     0.0; the choice is the first strict maximum over ascending actions, from lowest();
+//   node values from 0.0 in child order: terminal = return of b; chance and other player: sum of prob * V(child);
+//     b's own node: sum over ALL children of V(child) * (1.0 at the chosen action, else 0.0).
+// The evaluated policy at a decision edge with table index pi below a node with na children.
+__device__ __forceinline__ double cfr_br_evaluated(const CfrDev& d, int pi, int na, bool uniform) {
+  return uniform ? __ddiv_rn(1.0, (double)na) : d.cur_policy[pi];
+}
+
+__global__ void __launch_bounds__(1024) k_cfr_br(CfrDev d, CfrBrDev br, int iters, int iteration0) {
+  const int tid = threadIdx.x, nt = blockDim.x, N = d.n_nodes, L = d.n_levels;
+  for (int it = 0; it < iters; ++it) {
+    const double iteration = (double)(iteration0 + it + 1);          // ++iteration_ (cfr_br.cc:51)
+    const bool uniform = iteration0 + it == 0;                        // SetPolicy is skipped while iteration_ == 1
+    // (1a) counterfactual reach of every history for the player acting there.  The deepest level holds terminals only, so
+    // the barrier closing its level step below orders these writes before the first read.
+    for (int hh = tid; hh < d.n_hist; hh += nt) {
+      const int h = d.hist[hh], b = d.actor[h];
+      double acc = 1.0;
+      for (int n = h; n > 0; n = d.parent[n]) {
+        const int pi = d.policy_index[n];
+        if (pi < 0) acc = __dmul_rn(d.chance_prob[n], acc);
+        else if (d.par_actor[n] != b) acc = __dmul_rn(cfr_br_evaluated(d, pi, d.nchild[d.parent[n]], uniform), acc);
+      }
+      br.cf_reach[hh] = acc;
+    }
+    // (1b) both best responses, bottom-up, one level step each: a responder's node gets its value from the thread of its
+    // information state, which first chooses the action from the children's values; every other node from its children.
+    for (int l = L - 1; l >= 0; --l) {
+      for (int n = d.level_off[l] + tid; n < d.level_off[l + 1]; n += nt) {
+        const int kind = d.kind[n], fc = d.first_child[n], nc = d.nchild[n];
+        for (int b = 0; b < 2; ++b) {
+          if (kind == 2 && d.actor[n] == b) continue;
+          const double* V = br.value + b * N;
+          double v;
+          if (kind == 0) v = d.ret[2 * n + b];
+          else {
+            v = 0.0;
+            for (int c = 0; c < nc; ++c) {
+              const double pr = kind == 1 ? d.chance_prob[fc + c] : cfr_br_evaluated(d, d.policy_index[fc + c], nc, uniform);
+              v = __dadd_rn(v, __dmul_rn(pr, V[fc + c]));
+            }
+          }
+          br.value[b * N + n] = v;
+        }
+      }
+      for (int I = tid; I < d.n_infosets; I += nt) {
+        if (d.is_level[I] != l) continue;
+        const int b = d.is_player[I], na = d.is_off[I + 1] - d.is_off[I], h0 = d.hist_off[I], h1 = d.hist_off[I + 1];
+        double* V = br.value + b * N;
+        int arg = 0;
+        double best_value = -DBL_MAX;
+        for (int a = 0; a < na; ++a) {
+          double q = 0.0;
+          for (int hh = h0; hh < h1; ++hh) q = __dadd_rn(q, __dmul_rn(br.cf_reach[hh], V[d.first_child[d.hist[hh]] + a]));
+          if (q > best_value) { best_value = q; arg = a; }
+        }
+        br.best[I] = arg;
+        for (int hh = h0; hh < h1; ++hh) {
+          const int h = d.hist[hh], fc = d.first_child[h];
+          double v = 0.0;
+          for (int a = 0; a < na; ++a) v = __dadd_rn(v, __dmul_rn(V[fc + a], a == arg ? 1.0 : 0.0));
+          V[h] = v;
+        }
+      }
+      __syncthreads();
+    }
+    // (2) traversal t = p: p follows the current policy, the other player its best response (cfr.cc:371-377 overrides).
+    cfr_level_passes<2>(d, tid, nt, [&](const CfrDev& g, int n, int t) {
+      const int pi = g.policy_index[n];
+      if (pi < 0) return g.chance_prob[n];
+      if (g.par_actor[n] == t) return g.cur_policy[pi];
+      return br.best[g.infoset[g.parent[n]]] == g.aidx[n] ? 1.0 : 0.0;
+    });
+    // (3) each information state's update from its player's traversal, then regret matching (ApplyRegretMatching after both
+    // traversals: every read of the current policy above is behind the last level step's barrier).
+    for (int I = tid; I < d.n_infosets; I += nt) {
+      const int p = d.is_player[I], off = d.is_off[I], na = d.is_off[I + 1] - off;
+      CfrDev dp = d;
+      dp.reach += 2 * p * N; dp.value += 2 * p * N;
+      for (int hh = d.hist_off[I]; hh < d.hist_off[I + 1]; ++hh)
+        cfr_contribution(dp, d.hist[hh], p, off, na, 0, iteration,
+                         [&](int a, double regret) { d.regrets[off + a] = __dadd_rn(d.regrets[off + a], regret); },
+                         [&](int a, double inc) { d.cum_policy[off + a] = __dadd_rn(d.cum_policy[off + a], inc); });
+      cfr_update_policy(d, off, na, 0);
+    }
+    __syncthreads();
   }
 }
 
@@ -206,6 +310,8 @@ __global__ void __launch_bounds__(1024) k_cfr_nashconv(CfrDev d, int use_average
 
 using namespace b2s;
 
+static const char kNoShardedCfrBr[] = "cfr: a CFR-BR solver (B2S_CFR_BEST_RESPONSE_OPPONENTS) has no sharded iteration";
+
 extern "C" {
 
 int b2s_cfr_iterate(void* solver, int iters, void* stream) {
@@ -214,6 +320,12 @@ int b2s_cfr_iterate(void* solver, int iters, void* stream) {
   CfrSolver* S = (CfrSolver*)solver;
   B2S_CU(cudaSetDevice(S->device));
   if (iters == 0) return 0;
+  if (S->best_response_opponents) {
+    k_cfr_br<<<1, 1024, 0, (cudaStream_t)stream>>>(S->d, S->br, iters, S->iteration);
+    ++g_launches;
+    S->iteration += iters;
+    return launch_status("k_cfr_br launch");
+  }
   k_cfr<<<1, 1024, 0, (cudaStream_t)stream>>>(S->d, iters, S->iteration, S->linear_averaging, S->rm_plus);
   ++g_launches;
   S->iteration += iters;
@@ -226,6 +338,7 @@ int b2s_cfr_traverse_shard(void* solver, int player, int iteration, int shard, i
   if (!solver) return fail("cfr: null solver");
   if (player < 0 || player > 1 || num_shards < 1 || shard < 0 || shard >= num_shards) return fail("cfr: bad shard arguments");
   CfrSolver* S = (CfrSolver*)solver;
+  if (S->best_response_opponents) return fail(kNoShardedCfrBr);
   B2S_CU(cudaSetDevice(S->device));
   k_cfr_traverse<<<1, 1024, 0, (cudaStream_t)stream>>>(S->d, player, iteration, 0, S->linear_averaging, shard, num_shards);
   ++g_launches;
@@ -237,6 +350,7 @@ int b2s_cfr_traverse_shard(void* solver, int player, int iteration, int shard, i
 int b2s_cfr_apply_deltas(void* solver, void* stream) {
   if (!solver) return fail("cfr: null solver");
   CfrSolver* S = (CfrSolver*)solver;
+  if (S->best_response_opponents) return fail(kNoShardedCfrBr);
   B2S_CU(cudaSetDevice(S->device));
   k_cfr_apply<<<1, 1024, 0, (cudaStream_t)stream>>>(S->d, S->last_shard_player, S->rm_plus);
   ++g_launches;
@@ -322,6 +436,7 @@ int b2s_cfr_iterate_sharded(void* solver, int iters, void* stream) {
   if (!solver) return fail("cfr: null solver");
   if (iters < 0) return fail("cfr: negative iteration count");
   CfrSolver* S = (CfrSolver*)solver;
+  if (S->best_response_opponents) return fail(kNoShardedCfrBr);
   if (!S->comm) return fail("cfr: no communicator (b2s_cfr_comm_init / b2s_cfr_comm_adopt first)");
   B2S_CU(cudaSetDevice(S->device));
   if (iters == 0) return 0;

@@ -250,7 +250,17 @@ static int upload_tree(CfrSolver* S, const HostTree& t, const FlatTree& f) {
   TRY(upload(S, f.mc_node, &d.mc_node)); TRY(upload(S, f.entry_player, &d.entry_player));
   TRY(upload(S, f.policy_index, &d.policy_index)); TRY(upload(S, f.par_actor, &d.par_actor));
   TRY(upload(S, f.chance_reach, &d.chance_reach)); TRY(upload(S, f.is_level, &d.is_level));
-  TRY(alloc_d(S, 2 * (size_t)N, &d.reach)); TRY(alloc_d(S, N, &d.edge_prob)); TRY(alloc_d(S, 2 * (size_t)N, &d.value));
+  const size_t traversals = S->best_response_opponents ? 2 : 1;      // CFR-BR runs both players' traversals at once
+  TRY(alloc_d(S, 2 * traversals * N, &d.reach)); TRY(alloc_d(S, traversals * N, &d.edge_prob));
+  TRY(alloc_d(S, 2 * traversals * N, &d.value));
+  if (S->best_response_opponents) {
+    TRY(alloc_d(S, (size_t)d.n_hist, &S->br.cf_reach)); TRY(alloc_d(S, 2 * (size_t)N, &S->br.value));
+    void* best = nullptr;
+    B2S_CU(cudaMalloc(&best, sizeof(int) * (I ? I : 1)));
+    S->allocs.push_back(best);
+    B2S_CU(cudaMemset(best, 0, sizeof(int) * (I ? I : 1)));
+    S->br.best = (int*)best;
+  }
   TRY(alloc_d(S, E, &d.regrets)); TRY(alloc_d(S, E, &d.cum_policy)); TRY(alloc_d(S, E, &d.cur_policy));
   TRY(alloc_d(S, 2 * (size_t)d.n_contrib, &d.delta));
   {
@@ -288,6 +298,10 @@ int b2s_cfr_create(int game_id, const b2s_params* params, int flags, int device,
   if (gi.num_players != 2) return fail("cfr: two-player games only");
   if (gi.information_state_tensor_size <= 0)
     return fail("cfr: the game provides no information-state tensor (device CFR keys information states by it)");
+  const int br = (flags & B2S_CFR_BEST_RESPONSE_OPPONENTS) ? 1 : 0;
+  if (br && (flags & (B2S_CFR_LINEAR_AVERAGING | B2S_CFR_REGRET_MATCHING_PLUS | B2S_CFR_MCCFR_TABLES)))
+    return fail("cfr: B2S_CFR_BEST_RESPONSE_OPPONENTS (CFRBRSolver) takes no other flag: it averages plainly, without RM+, "
+                "on CFR tables");
   HostTree t;
   FlatTree f;
   TRY(expand_tree(game_id, params, device, gi, t));
@@ -297,10 +311,17 @@ int b2s_cfr_create(int game_id, const b2s_params* params, int flags, int device,
   S->linear_averaging = (flags & B2S_CFR_LINEAR_AVERAGING) ? 1 : 0;
   S->rm_plus = (flags & B2S_CFR_REGRET_MATCHING_PLUS) ? 1 : 0;
   S->mccfr_tables = (flags & B2S_CFR_MCCFR_TABLES) ? 1 : 0;
+  S->best_response_opponents = br;
   S->is_player = std::move(t.is_player); S->is_off = std::move(t.is_off); S->legal_actions = std::move(t.legal_actions);
   S->node_counts = std::move(t.node_counts); S->keys = std::move(t.keys);
   S->mc_cap_es = f.cap_es; S->mc_cap_os = f.cap_os;
   for (size_t i = 0; i + 1 < S->is_off.size(); ++i) S->max_actions = std::max(S->max_actions, S->is_off[i + 1] - S->is_off[i]);
+  // CFR-BR sums children in the device's child order where the reference's best response iterates its btree_map of
+  // actions: both are ascending only when every information state lists its legal actions in ascending order.
+  if (br)
+    for (size_t i = 0; i + 1 < S->is_off.size(); ++i)
+      for (int k = S->is_off[i] + 1; k < S->is_off[i + 1]; ++k)
+        if (S->legal_actions[k] <= S->legal_actions[k - 1]) return fail("cfr: CFR-BR needs legal actions in ascending order");
   B2S_CU(cudaSetDevice(device));
   TRY(upload_tree(S.get(), t, f));
   *out_solver = S.release();

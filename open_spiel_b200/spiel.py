@@ -894,13 +894,14 @@ class CFRSolver:
     """Mirror of pyspiel.CFRSolver(game) (python/pybind11/policy.cc:224-245; algorithms/cfr.h:312-328) with
     device-resident tables.  CFRPlusSolver = CFRSolver(game, linear_averaging=True, regret_matching_plus=True)."""
 
-    def __init__(self, game, linear_averaging=False, regret_matching_plus=False, _mccfr_tables=False):
+    def __init__(self, game, linear_averaging=False, regret_matching_plus=False, _mccfr_tables=False, _best_response_opponents=False):
         from ._lib import CfrInfo
         if not torch.cuda.is_available():
             raise B2SError("no CUDA device: open_spiel_b200 has no CPU fallback")
         self.game = game
         self._h = C.c_void_p()
-        flags = (1 if linear_averaging else 0) | (2 if regret_matching_plus else 0) | (4 if _mccfr_tables else 0)
+        flags = ((1 if linear_averaging else 0) | (2 if regret_matching_plus else 0) | (4 if _mccfr_tables else 0)
+                 | (8 if _best_response_opponents else 0))
         self._plus = bool(linear_averaging and regret_matching_plus)
         check(lib().b2s_cfr_create(game._gid, C.byref(game._cparams), flags, game.device, C.byref(self._h)))
         self._info = CfrInfo()
@@ -958,7 +959,7 @@ class CFRSolver:
         from . import serialization as ser
         t = self.table()
         i = self.info()
-        kind = "CFRPlusSolver" if getattr(self, "_plus", False) else "CFRSolver"
+        kind = self._solver_type or ("CFRPlusSolver" if getattr(self, "_plus", False) else "CFRSolver")
         return ser.serialize_cfr_solver(str(self.game), kind, i.iteration, ser.table_keys(self.game._name, t), t, delimiter)
 
     def load_serialized(self, text, delimiter="<~>"):
@@ -971,6 +972,7 @@ class CFRSolver:
         return parsed
 
     _has_current_policy = True
+    _solver_type = None         # the [SolverType] serialize() writes, when the flags alone do not name it
 
     def _require_current_policy(self):
         if not self._has_current_policy:
@@ -1039,6 +1041,30 @@ class CFRSolver:
             probs = [1.0 / (hi - lo)] * (hi - lo) if s == 0.0 else [v / s for v in cp]
             pol[t["keys"][k].tobytes()] = list(zip(t["legal_actions"][lo:hi].tolist(), probs))
         return pol
+
+
+class CFRBRSolver(CFRSolver):
+    """Mirror of pyspiel.CFRBRSolver(game) (python/pybind11/policy.cc:264-280; algorithms/cfr_br.h) with device-resident
+    tables: each iteration both players' pure best responses to the current policy (the uniform policy on iteration 1), then
+    each player's traversal against the other's best response, then regret matching.  Tables match the reference bit for
+    bit; see B2S_CFR_BEST_RESPONSE_OPPONENTS in include/b2s.h."""
+
+    _solver_type = "CFRBRSolver"
+
+    def __init__(self, game):
+        super().__init__(game, _best_response_opponents=True)
+
+    def evaluate_and_update_policy(self, iterations=1):
+        """CFRBRSolver::EvaluateAndUpdatePolicy (cfr_br.cc:50-82), `iterations` times in one kernel launch."""
+        super().evaluate_and_update_policy(iterations)
+
+    def load_serialized(self, text, delimiter="<~>"):
+        """Load a CFRBRSolver Serialize text (ours or the reference's), as DeserializeCFRBRSolver (cfr_br.cc:84-96)."""
+        from . import serialization as ser
+        kind = ser.deserialize_cfr_solver(text, delimiter)["solver_type"]
+        if kind != "CFRBRSolver":
+            raise B2SError("CFRBRSolver.load_serialized: the text holds a %r, not a CFRBRSolver" % kind)
+        return super().load_serialized(text, delimiter)
 
 
 class ExternalSamplingMCCFRSolver(CFRSolver):
