@@ -441,6 +441,21 @@ enum { B2S_CFR_LINEAR_AVERAGING = 1, B2S_CFR_REGRET_MATCHING_PLUS = 2,   /* both
  * Averaging is plain and there is no RM+: the flag combined with any other is an error.  Tables match the reference's
  * CFRBRSolver bit for bit.  b2s_cfr_traverse_shard, b2s_cfr_apply_deltas and b2s_cfr_iterate_sharded refuse such a solver;
  * export, import, NashConv, best response, tables and set_iteration work as on any CFR solver. */
+/* b2s_dcfr_create: a CFR solver on which b2s_cfr_iterate runs Discounted CFR, the reference's
+ * python/algorithms/discounted_cfr.py DCFRSolver(game, alpha, beta, gamma) (LCFRSolver = alpha = beta = gamma = 1):
+ * alternating updates; per iteration t and player p, p's traversal with average-policy increments (reach * pi) * t**gamma,
+ * then p's regrets multiplied by t**alpha / (t**alpha + 1) where >= 0 (-0.0 included) and by t**beta / (t**beta + 1)
+ * elsewhere, then regret matching of the whole table.  Decision nodes no player reaches are pruned as the reference prunes
+ * them.  The factors are computed on the host in double with std::pow (glibc pow, which CPython's float ** calls) from
+ * the absolute iteration t, so a table imported at iteration k continues with t = k + 1.  They are read from a device
+ * window of at least 65,536 and at most 2**20 iterations (24 B each), rebuilt when a launch leaves it; a call of more than
+ * 2**20 iterations is enqueued as several launches.  The window is allocated and freed in the order of `stream`, so calls
+ * on one solver must be ordered (one stream, or streams the caller orders), as its tables require anyway.  For
+ * integral exponents the reference computes t**k in Python ints; both agree bit for bit while t**k + 1 <= 2**53 (gamma = 2:
+ * t <= 94,906,265).  Tables match the reference bit for bit, the sign of zero included.  Non-finite alpha, beta or gamma
+ * are an error; b2s_cfr_iterate refuses a negative iteration counter and one it would carry past INT_MAX.  b2s_cfr_traverse_shard, b2s_cfr_apply_deltas,
+ * b2s_cfr_iterate_sharded and the MCCFR iterate calls refuse such a solver; export, import, NashConv, best response,
+ * tables and set_iteration work as on any CFR solver. */
 typedef struct b2s_cfr_info {
   int32_t num_nodes, num_levels, num_infosets, num_entries;   /* entries = sum of legal actions over infosets */
   int32_t key_floats;                                         /* information-state tensor size */
@@ -449,6 +464,8 @@ typedef struct b2s_cfr_info {
   int32_t reserved[3];
 } b2s_cfr_info;
 int  b2s_cfr_create(int game_id, const b2s_params* params, int flags, int device, void** out_solver);
+int  b2s_dcfr_create(int game_id, const b2s_params* params, double alpha, double beta, double gamma, int device,
+                     void** out_solver);
 void b2s_cfr_destroy(void* solver);
 /* `iters` x CFRSolverBase::EvaluateAndUpdatePolicy, enqueued on `stream`. */
 int  b2s_cfr_iterate(void* solver, int iters, void* stream);

@@ -6,5 +6,5 @@ extension (Game.new_batch -> BatchedState) that the kernels exist for.  All comp
 C ABI in include/b2s.h (libb2s.so); torch is used only for device buffers and streams.
 """
 from ._lib import B2SError as SpielError  # noqa: F401
-from .spiel import (AlphaBetaEvalSearch, BatchedState, BatchedTrajectory, CFRBRSolver, CFRSolver, ChildSelectionPolicy, ExternalSamplingMCCFRSolver, OutcomeSamplingMCCFRSolver, Game, ObservationType, StepType, VectorEnv, VectorTimeStep, MCTSBot, MCTSEvalSearch, RandomRolloutEvaluator, State, load_game, bind_host_to_device, mcts_nodes_used,
+from .spiel import (AlphaBetaEvalSearch, BatchedState, BatchedTrajectory, CFRBRSolver, CFRSolver, ChildSelectionPolicy, DCFRSolver, LCFRSolver, ExternalSamplingMCCFRSolver, OutcomeSamplingMCCFRSolver, Game, ObservationType, StepType, VectorEnv, VectorTimeStep, MCTSBot, MCTSEvalSearch, RandomRolloutEvaluator, State, load_game, bind_host_to_device, mcts_nodes_used,
                     alpha_beta_search, alpha_beta_search_evaluated, dirichlet_noise, mcts_search, mcts_search_evaluated, registered_names)  # noqa: F401

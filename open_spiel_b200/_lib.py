@@ -122,6 +122,7 @@ SIGNATURES = {
     "b2s_alpha_beta_eval_results": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "b2s_alpha_beta_eval_destroy": (None, [_VP]),
     "b2s_cfr_create": (C.c_int, [C.c_int, C.POINTER(Params), C.c_int, C.c_int, C.POINTER(_VP)]),
+    "b2s_dcfr_create": (C.c_int, [C.c_int, C.POINTER(Params), C.c_double, C.c_double, C.c_double, C.c_int, C.POINTER(_VP)]),
     "b2s_cfr_destroy": (None, [_VP]),
     "b2s_cfr_iterate": (C.c_int, [_VP, C.c_int, _VP]),
     "b2s_cfr_info_get": (C.c_int, [_VP, C.POINTER(CfrInfo)]),

@@ -1,7 +1,11 @@
 // Full-width CFR (single-GPU persistent kernel and the sharded / NCCL iteration) and NashConv / best response on the
 // flattened tree of cfr_tree.cu.  Floating-point conventions: cfr.cuh.
 #include <float.h>
+#include <limits.h>
 #include <string.h>
+
+#include <algorithm>
+#include <cmath>
 
 #include "cfr.cuh"
 
@@ -166,6 +170,59 @@ __global__ void __launch_bounds__(1024) k_cfr_br(CfrDev d, CfrBrDev br, int iter
   }
 }
 
+// ---- Discounted CFR (python/algorithms/discounted_cfr.py:190-209, _DCFRSolver.evaluate_and_update_policy) -----------
+// Per iteration t, for p = 0, 1: (1) player p's traversal (:93-188): cfr.py's values, reach and regrets, the average-policy
+// increment (reach * pi) * w_t (:181-184); (2) every regret of p's information states multiplied by pos_t where it is >= 0
+// (so -0.0 too) and by neg_t elsewhere (:199-209); (3) regret matching of the whole table (cfr.py:78-98), which player 1's
+// traversal then follows.  factors[3 k ...] = (pos_t, neg_t, w_t) of iteration t = base + 1 + k, computed on the host
+// (dcfr_factors).
+//
+// The reference prunes decision nodes no player reaches (:132-133): it returns zeros there and updates nothing below.
+// Under DCFR that decides bits: a regret left alone by ~1,075 halvings of beta = 0 is -0.0, and adding the +0.0 or -0.0 of
+// a zero-reach contribution flips it or not.  So k_dcfr adds nothing at such histories and takes every other
+// contribution, 0 * (V(child) - v) included, from the reference's pruned values.  Those need each node's reach before its
+// value: the reach sweep runs to the bottom first, then the value sweep (2L - 1 level steps where cfr_level_passes takes
+// L).  Only nodes no player reaches get other values than the fused sweep's; they sit below a zero-probability edge, which
+// wipes the difference out of every value above them.
+__global__ void __launch_bounds__(1024) k_dcfr(CfrDev d, const double* factors, int iters, int iteration0, int base) {
+  const int tid = threadIdx.x, nt = blockDim.x, L = d.n_levels, N = d.n_nodes;
+  for (int it = 0; it < iters; ++it) {
+    const double* f = factors + 3 * ((size_t)(iteration0 - base) + it);   // t = iteration0 + it + 1: self._iteration += 1 (:192)
+    const double pos = f[0], neg = f[1], w = f[2];
+    for (int p = 0; p < 2; ++p) {
+      for (int n = 1 + tid; n < N; n += nt) d.edge_prob[n] = CurrentPolicyEdge{}(d, n, 0);
+      if (tid == 0) { d.reach[0] = 1.0; d.reach[1] = 1.0; }
+      __syncthreads();
+      for (int l = 1; l < L; ++l) {
+        for (int n = d.level_off[l] + tid; n < d.level_off[l + 1]; n += nt) cfr_reach_step<1>(d, N, n);
+        __syncthreads();
+      }
+      for (int l = L - 1; l >= 0; --l) {
+        for (int n = d.level_off[l] + tid; n < d.level_off[l + 1]; n += nt) cfr_value_step<1, true>(d, N, n);
+        __syncthreads();
+      }
+      for (int I = tid; I < d.n_infosets; I += nt) {
+        const int off = d.is_off[I], na = d.is_off[I + 1] - off;
+        if (d.is_player[I] == p) {
+          for (int hh = d.hist_off[I]; hh < d.hist_off[I + 1]; ++hh) {
+            const int h = d.hist[hh];
+            if (d.reach[2 * h] == 0.0 && d.reach[2 * h + 1] == 0.0) continue;
+            cfr_contribution(d, h, p, off, na, 0, 0.0,
+                             [&](int a, double regret) { d.regrets[off + a] = __dadd_rn(d.regrets[off + a], regret); },
+                             [&](int a, double inc) { d.cum_policy[off + a] = __dadd_rn(d.cum_policy[off + a], __dmul_rn(inc, w)); });
+          }
+          for (int a = 0; a < na; ++a) {
+            const double r = d.regrets[off + a];
+            d.regrets[off + a] = __dmul_rn(r, r >= 0 ? pos : neg);
+          }
+        }
+        regret_matching(d.regrets + off, d.cur_policy + off, na);
+      }
+      __syncthreads();
+    }
+  }
+}
+
 // ---- multi-GPU variant: one traversal split into "my shard's contributions" / all-reduce / "apply in order" ---------
 // Every rank runs the level passes of the whole (tiny) tree; history slot hh's regret and average-policy contributions
 // (one pair per action, the very expressions of k_cfr above) are written by rank (hh mod num_shards) into the
@@ -311,6 +368,37 @@ __global__ void __launch_bounds__(1024) k_cfr_nashconv(CfrDev d, int use_average
 using namespace b2s;
 
 static const char kNoShardedCfrBr[] = "cfr: a CFR-BR solver (B2S_CFR_BEST_RESPONSE_OPPONENTS) has no sharded iteration";
+static const char kNoShardedDcfr[] = "cfr: a DCFR solver (b2s_dcfr_create) has no sharded iteration";
+
+constexpr int kDcfrLaunch = 1 << 20;     // most iterations one k_dcfr launch runs: bounds the factor window
+constexpr int kDcfrWindow = 1 << 16;     // fewest iterations a factor window covers
+
+// Makes S->dcfr_factors cover iterations first + 1 .. first + n: (t**alpha / (t**alpha + 1), t**beta / (t**beta + 1),
+// t**gamma) as discounted_cfr.py computes them, std::pow being glibc's pow as CPython's float ** is.  A window that does
+// not cover them is replaced by one starting at first + 1, of max(n, kDcfrWindow) entries (at most 24 MiB), allocated,
+// filled and the old one freed in the order of `st`: launches that read the old window were enqueued before this call,
+// and calls on one solver are ordered (b2s.h), so none of them can still be reading it when it is freed.
+static int dcfr_factors(CfrSolver* S, int first, int n, cudaStream_t st) {
+  if (S->dcfr_factors && first >= S->dcfr_base && (long long)first + n <= (long long)S->dcfr_base + S->dcfr_capacity) return 0;
+  const int cap = std::max(n, kDcfrWindow);
+  std::vector<double> h(3 * (size_t)cap);
+  for (long long k = 0; k < cap; ++k) {
+    const double t = (double)(first + 1 + k);
+    const double ta = std::pow(t, S->dcfr_alpha), tb = std::pow(t, S->dcfr_beta);
+    h[3 * k] = ta / (ta + 1.0);
+    h[3 * k + 1] = tb / (tb + 1.0);
+    h[3 * k + 2] = std::pow(t, S->dcfr_gamma);
+  }
+  void* p = nullptr;
+  B2S_CU(cudaMallocAsync(&p, sizeof(double) * h.size(), st));
+  const cudaError_t e = cudaMemcpyAsync(p, h.data(), sizeof(double) * h.size(), cudaMemcpyHostToDevice, st);  // pageable: staged before return
+  if (e != cudaSuccess) { cudaFreeAsync(p, st); return cuda_fail(e, "dcfr: factor window"); }
+  if (S->dcfr_factors) B2S_CU(cudaFreeAsync(S->dcfr_factors, st));
+  S->dcfr_factors = (double*)p;
+  S->dcfr_base = first;
+  S->dcfr_capacity = cap;
+  return 0;
+}
 
 extern "C" {
 
@@ -320,6 +408,20 @@ int b2s_cfr_iterate(void* solver, int iters, void* stream) {
   CfrSolver* S = (CfrSolver*)solver;
   B2S_CU(cudaSetDevice(S->device));
   if (iters == 0) return 0;
+  if (S->dcfr) {
+    if (S->iteration < 0 || iters > INT_MAX - S->iteration)
+      return fail("dcfr: the iteration counter must stay within [0, INT_MAX]");
+    for (int left = iters; left > 0;) {
+      const int n = std::min(left, kDcfrLaunch);
+      if (int r = dcfr_factors(S, S->iteration, n, (cudaStream_t)stream)) return r;
+      k_dcfr<<<1, 1024, 0, (cudaStream_t)stream>>>(S->d, S->dcfr_factors, n, S->iteration, S->dcfr_base);
+      ++g_launches;
+      if (int r = launch_status("k_dcfr launch")) return r;
+      S->iteration += n;
+      left -= n;
+    }
+    return 0;
+  }
   if (S->best_response_opponents) {
     k_cfr_br<<<1, 1024, 0, (cudaStream_t)stream>>>(S->d, S->br, iters, S->iteration);
     ++g_launches;
@@ -339,6 +441,7 @@ int b2s_cfr_traverse_shard(void* solver, int player, int iteration, int shard, i
   if (player < 0 || player > 1 || num_shards < 1 || shard < 0 || shard >= num_shards) return fail("cfr: bad shard arguments");
   CfrSolver* S = (CfrSolver*)solver;
   if (S->best_response_opponents) return fail(kNoShardedCfrBr);
+  if (S->dcfr) return fail(kNoShardedDcfr);
   B2S_CU(cudaSetDevice(S->device));
   k_cfr_traverse<<<1, 1024, 0, (cudaStream_t)stream>>>(S->d, player, iteration, 0, S->linear_averaging, shard, num_shards);
   ++g_launches;
@@ -351,6 +454,7 @@ int b2s_cfr_apply_deltas(void* solver, void* stream) {
   if (!solver) return fail("cfr: null solver");
   CfrSolver* S = (CfrSolver*)solver;
   if (S->best_response_opponents) return fail(kNoShardedCfrBr);
+  if (S->dcfr) return fail(kNoShardedDcfr);
   B2S_CU(cudaSetDevice(S->device));
   k_cfr_apply<<<1, 1024, 0, (cudaStream_t)stream>>>(S->d, S->last_shard_player, S->rm_plus);
   ++g_launches;
@@ -437,6 +541,7 @@ int b2s_cfr_iterate_sharded(void* solver, int iters, void* stream) {
   if (iters < 0) return fail("cfr: negative iteration count");
   CfrSolver* S = (CfrSolver*)solver;
   if (S->best_response_opponents) return fail(kNoShardedCfrBr);
+  if (S->dcfr) return fail(kNoShardedDcfr);
   if (!S->comm) return fail("cfr: no communicator (b2s_cfr_comm_init / b2s_cfr_comm_adopt first)");
   B2S_CU(cudaSetDevice(S->device));
   if (iters == 0) return 0;

@@ -3,6 +3,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <memory>
 #include <unordered_map>
 
@@ -325,6 +326,18 @@ int b2s_cfr_create(int game_id, const b2s_params* params, int flags, int device,
   B2S_CU(cudaSetDevice(device));
   TRY(upload_tree(S.get(), t, f));
   *out_solver = S.release();
+  return 0;
+}
+
+int b2s_dcfr_create(int game_id, const b2s_params* params, double alpha, double beta, double gamma, int device,
+                    void** out_solver) {
+  if (!out_solver) return fail("dcfr: null out_solver");
+  *out_solver = nullptr;
+  if (!std::isfinite(alpha) || !std::isfinite(beta) || !std::isfinite(gamma))
+    return fail("dcfr: alpha, beta and gamma must be finite");
+  TRY(b2s_cfr_create(game_id, params, 0, device, out_solver));
+  CfrSolver* S = (CfrSolver*)*out_solver;
+  S->dcfr = 1; S->dcfr_alpha = alpha; S->dcfr_beta = beta; S->dcfr_gamma = gamma;
   return 0;
 }
 

@@ -894,7 +894,8 @@ class CFRSolver:
     """Mirror of pyspiel.CFRSolver(game) (python/pybind11/policy.cc:224-245; algorithms/cfr.h:312-328) with
     device-resident tables.  CFRPlusSolver = CFRSolver(game, linear_averaging=True, regret_matching_plus=True)."""
 
-    def __init__(self, game, linear_averaging=False, regret_matching_plus=False, _mccfr_tables=False, _best_response_opponents=False):
+    def __init__(self, game, linear_averaging=False, regret_matching_plus=False, _mccfr_tables=False, _best_response_opponents=False,
+                 _dcfr=None):
         from ._lib import CfrInfo
         if not torch.cuda.is_available():
             raise B2SError("no CUDA device: open_spiel_b200 has no CPU fallback")
@@ -903,7 +904,11 @@ class CFRSolver:
         flags = ((1 if linear_averaging else 0) | (2 if regret_matching_plus else 0) | (4 if _mccfr_tables else 0)
                  | (8 if _best_response_opponents else 0))
         self._plus = bool(linear_averaging and regret_matching_plus)
-        check(lib().b2s_cfr_create(game._gid, C.byref(game._cparams), flags, game.device, C.byref(self._h)))
+        if _dcfr is None:
+            check(lib().b2s_cfr_create(game._gid, C.byref(game._cparams), flags, game.device, C.byref(self._h)))
+        else:                   # (alpha, beta, gamma) of a DCFRSolver
+            check(lib().b2s_dcfr_create(game._gid, C.byref(game._cparams), *[float(x) for x in _dcfr], game.device,
+                                        C.byref(self._h)))
         self._info = CfrInfo()
         check(lib().b2s_cfr_info_get(self._h, C.byref(self._info)))
 
@@ -1065,6 +1070,37 @@ class CFRBRSolver(CFRSolver):
         if kind != "CFRBRSolver":
             raise B2SError("CFRBRSolver.load_serialized: the text holds a %r, not a CFRBRSolver" % kind)
         return super().load_serialized(text, delimiter)
+
+
+class DCFRSolver(CFRSolver):
+    """Mirror of python/algorithms/discounted_cfr.py DCFRSolver(game, alpha=3/2, beta=0, gamma=2) with device-resident
+    tables (k_dcfr): alternating updates; per iteration t and player, the traversal with average-policy increments
+    (reach * pi) * t**gamma, then the player's regrets multiplied by t**alpha / (t**alpha + 1) where >= 0 and by
+    t**beta / (t**beta + 1) elsewhere, then regret matching.  Tables match the reference bit for bit; see b2s_dcfr_create
+    in include/b2s.h.  average_policy() is cfr.py's _update_average_policy, which is CFRAveragePolicy's rule."""
+
+    def __init__(self, game, alpha=3 / 2, beta=0, gamma=2):
+        self.alpha, self.beta, self.gamma = alpha, beta, gamma
+        super().__init__(game, _dcfr=(alpha, beta, gamma))
+
+    def evaluate_and_update_policy(self, iterations=1):
+        """_DCFRSolver.evaluate_and_update_policy (discounted_cfr.py:190-209), `iterations` times in one kernel launch."""
+        super().evaluate_and_update_policy(iterations)
+
+    _NO_TEXT = "%s.%s: no text format: the reference's DCFR has none, and CFRSolver text would resume as plain CFR"
+
+    def serialize(self, delimiter="<~>"):
+        raise B2SError(self._NO_TEXT % (type(self).__name__, "serialize"))
+
+    def load_serialized(self, text, delimiter="<~>"):
+        raise B2SError(self._NO_TEXT % (type(self).__name__, "load_serialized"))
+
+
+class LCFRSolver(DCFRSolver):
+    """Mirror of python/algorithms/discounted_cfr.py LCFRSolver(game): DCFRSolver with alpha = beta = gamma = 1."""
+
+    def __init__(self, game):
+        super().__init__(game, alpha=1, beta=1, gamma=1)
 
 
 class ExternalSamplingMCCFRSolver(CFRSolver):
